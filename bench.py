@@ -1,5 +1,5 @@
 #!/usr/bin/env python3
-"""bench.py - MCP tools/call transcodes/sec on B200 (BASELINE.json metric).
+"""bench.py - MCP tools/call transcodes/sec on the H100 (BASELINE.json metric).
 
 One step = one pass of the hot path over one synthetic batch: the request side (arguments JSON ->
 protobuf wire) followed by the reply side (protobuf wire -> protojson text) for every item.
@@ -10,6 +10,7 @@ them under `configs`, each with its own roofline entry.
 
   python bench.py [--gpus N] [--steps K] [--warmup W] [--workload nested|flat|blob|mixed] [--items M]
   python bench.py --impl reference ...      (the CPU path: oracle port on all host cores, same items)
+  python bench.py --dump-outputs DIR ...    (also writes what the last timed step computed as DIR/*.npy)
 
 Under torchrun (N > 1) every rank owns one GPU and its own shard of the batch (items shard by
 index, no collective on the data path); rank 0 prints one JSON line.
@@ -36,6 +37,7 @@ WORKLOAD_NAMES = {
     "mixed": "configs[4] mixed replay: 32 methods (4 of the reference's protos + 28 generated), method Zipf(1.1), size Zipf(1.2) 64B-64KiB",
 }
 DEFAULT_ITEMS = {"nested": 148 * 1024, "flat": 148 * 1024, "blob": 4096, "mixed": 128 * 1024}
+DUMP_BYTES = 64_000_000  # --dump-outputs writes at most this much
 METRIC = "tools_call_transcodes_per_sec"
 UNIT = "transcodes/s"
 # profile slot -> kernel function (for the ncu traffic table) and what it reads / writes
@@ -354,6 +356,39 @@ class Resident:
         barrier()
         return e0.elapsed_time(e1)
 
+    def dump_outputs(self, out_dir, prefix=""):
+        """what the last step handed back, per direction (request: wire bytes, reply: protojson text): the status and
+        output offsets of every item, and the output bytes of a fixed, seeded sample of items, one float32 per byte.
+        The inputs depend only on the arguments, so two builds can be compared file for file."""
+        torch = self.torch
+        torch.cuda.synchronize()
+        n = self.n
+        sides = [("reply", self.d_rep_out, self.d_rep_out_off, self.d_rep_st)]
+        if self.have_req:
+            sides.insert(0, ("request", self.d_req_out, self.d_req_out_off, self.d_req_st))
+        sample = np.sort(np.random.default_rng(0x5EED).choice(n, size=min(n, 2048), replace=False))
+        # every item's status and offsets when they take at most a quarter of the budget, else those of the sample
+        full = len(sides) * (4 * n + 8 * (n + 1)) <= DUMP_BYTES // 4
+        meta = 8 * len(sample) + len(sides) * ((4 * n + 8 * (n + 1)) if full else 12 * len(sample)) + 4096  # + .npy headers
+        byte_cap = (DUMP_BYTES - meta) // (4 * len(sides))
+        os.makedirs(out_dir, exist_ok=True)
+        arrays = {"sample_items": sample.astype(np.float64)}
+        for name, d_out, d_off, d_st in sides:
+            off = d_off.cpu().numpy().astype(np.int64)
+            st = d_st.cpu().numpy()
+            out = d_out[: int(off[n])].cpu().numpy()
+            if full:
+                arrays[name + "_status"] = st.astype(np.float32)
+                arrays[name + "_offsets"] = off.astype(np.float64)
+            else:
+                arrays[name + "_sample_status"] = st[sample].astype(np.float32)
+                arrays[name + "_sample_lengths"] = (off[sample + 1] - off[sample]).astype(np.float64)
+            # the sampled items' outputs back to back, cut at the byte budget
+            picked = np.concatenate([out[off[i]:off[i + 1]] for i in sample])
+            arrays[name + "_sample_bytes"] = picked[:byte_cap].astype(np.float32)
+        for k, a in arrays.items():
+            np.save(os.path.join(out_dir, prefix + k + ".npy"), a)
+
     def kernel_table(self):
         """per-kernel device time: the same kernels, same inputs, serialized on one stream so that each launch has the
         GPU to itself (CUDA events around every launch), with the bytes of the items each kernel actually takes"""
@@ -476,6 +511,7 @@ def main():
     ap.add_argument("--no-parity", action="store_true", help="skip the whole-batch comparison with the CPU oracle")
     ap.add_argument("--e2e-serial", action="store_true", help="end-to-end: request call, then reply call (default: both in flight)")
     ap.add_argument("--one-stream", action="store_true", help="serialize request and reply side on one stream")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed step's outputs to DIR/*.npy (float32 / float64, at most 64 MB)")
     args = ap.parse_args()
     if args.items == 0:
         args.items = DEFAULT_ITEMS[args.workload]
@@ -532,6 +568,8 @@ def main():
     sampler.start()
     ms = R.timed(args.steps, barrier, args.one_stream)
     clocks = sampler.stop()
+    if args.dump_outputs:
+        R.dump_outputs(args.dump_outputs, "rank%d_" % rank if world > 1 else "")
     launches = eng.launch_count() - launches0
     ms_max = max_ranks(ms)
     value = world * n * args.steps / (ms_max / 1000.0)
@@ -810,7 +848,7 @@ def roofline_of(kern, dom, workload, n, step_ms, J_in, W_in, W_out, J_out, with_
         peak = float(json.load(open(peaks_path))["hbm_gbs"])
         peak_src = "measured (MEASURED_PEAKS.json hbm_gbs, copy read+write)"
     else:
-        peak, peak_src = 6650.0, "fallback (B200_PROFILING.md)"
+        peak, peak_src = 3350.0, "H100 SXM data sheet HBM3 bandwidth (not measured)"
     if not dom:
         return None
     a = kern[dom]["gbs"] or 0.0

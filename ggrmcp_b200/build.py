@@ -1,4 +1,4 @@
-"""Builds libggrmcp_b200.so (sm_100a only) in-tree with nvcc.  No JIT, no other architectures.
+"""Builds libggrmcp_b200.so (sm_90a only, for the H100) in-tree with nvcc.  No JIT, no other architectures.
 
 One object per translation unit, compiled in parallel, then linked:
   ggr_engine.cu       host side of the C ABI + the block-sum scan kernel
@@ -20,7 +20,7 @@ OBJ = os.path.join(HERE, "build")
 LIB = os.path.join(HERE, "libggrmcp_b200.so")
 UNITS = ["ggr_engine.cu", "ggr_kernels_enc.cu", "ggr_kernels_dec.cu", "ggr_kernels_coop.cu", "ggr_kernels_coop_enc.cu", "ggr_kernels_walk.cu", "ggr_kernels_wrap.cu", "ggr_schema.cc"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC",
+FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC",
          "-I" + os.path.join(os.path.dirname(HERE), "include")]
 
 

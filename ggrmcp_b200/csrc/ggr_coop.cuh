@@ -20,7 +20,7 @@
 #pragma once
 #include "ggr_decode.cuh"
 #ifndef COOP_WORD_COPY_MIN
-#define COOP_WORD_COPY_MIN 24u /* reply write kernel: 1.04 -> 1.02 ms against 12 */
+#define COOP_WORD_COPY_MIN 24u /* reply write kernel: faster than 12 when tuned before the H100 port */
 #endif
 #include "ggr_warp.cuh"
 
@@ -77,10 +77,10 @@ struct CoopEnt {            // 32 bytes: saved between the passes as two 16-byte
 #define GGR_COOP_LONG_MAX 32u
 #endif
 #ifndef COOP_WIN_CACHE
-#define COOP_WIN_CACHE 0 /* 1: the scan keeps two 16-byte chunks in registers (measured: 1.76 -> 1.90 ms, not used) */
+#define COOP_WIN_CACHE 0 /* 1: the scan keeps two 16-byte chunks in registers (slower when tuned before the H100 port, not used) */
 #endif
 #ifndef COOP_COLD_LEAF
-#define COOP_COLD_LEAF 0 /* 1: float / timestamp sizing as a call (measured: 1.85 -> 1.90 ms, not used) */
+#define COOP_COLD_LEAF 0 /* 1: float / timestamp sizing as a call (slower when tuned before the H100 port, not used) */
 #endif
 #define GGR_COOP_DIRTY_MAX 64u
 template <int NE>
@@ -98,8 +98,8 @@ struct CoopSharedT {
   u16 dlist[GGR_COOP_DIRTY_MAX];          // strings that need escaping / validation: sized by the whole warp
 };
 typedef CoopSharedT<GGR_COOP_ENTRIES> CoopShared;      // first tier
-// second tier: replies of thousands of field occurrences (a 39 KB reply of the mixed replay holds 1 800: on one lane of the
-// per-thread kernels that is 40 ms per pass); 141 KB of shared memory = one warp per SM, the saved table goes to a pool
+// second tier: replies of thousands of field occurrences (a 39 KB reply of the mixed replay holds 1 800: one lane of the
+// per-thread kernels walks them one after the other); 141 KB of shared memory = one warp per SM, the saved table goes to a pool
 #define GGR_COOP_BIG_ENTRIES 4096
 typedef CoopSharedT<GGR_COOP_BIG_ENTRIES> CoopSharedBig;
 
@@ -597,7 +597,7 @@ GGR_DEV void coop_size_leaf(SH& S, const DecCtx& cx, u32 ei, bool have_masks) {
     n += c.pos;
   } else if (COOP_COLD_LEAF && (cls == DC_FLOAT || cls == DC_TS)) {
     // shortest-digits floats and timestamps: out of line, so that the size kernel's hot loop stays small (the kernel
-    // waited for instructions on 0.94 of its issue slots, profiles/ncu_r2_final_lockstep_kernels_151552items.csv)
+    // waits for instructions when its hot loop outgrows the instruction cache)
     const i32 v = coop_leaf_size_cold(cx, e, f);
     if (v < 0) {
       COOP_BAIL(S);
@@ -656,7 +656,7 @@ GGR_DEV void coop_offsets_message(SH& S, const DecCtx& cx, u32 me) {
 #define GGR_COOP_STAGE 8192u /* items with more text than this: per-thread kernels */
 #ifndef GGR_COOP_STAGE_BUF
 /* the writer's staging buffer; larger texts are written in place.  6144 (configs[2]: texts up to 6.0 KB) with the kernel
-   compiled for 7 blocks per SM (72 registers): 1.08 -> 1.00 ms; for 8 blocks (64 registers, spills) 1.11 ms */
+   compiled for 7 blocks per SM (72 registers); 8 blocks (64 registers) spilled when tuned before the H100 port */
 #define GGR_COOP_STAGE_BUF 6144u
 #endif
 struct
@@ -893,7 +893,7 @@ GGR_DEV int coop_write_item(CoopStage& E, const DecCtx& cx, const U4* tab, u32 n
   }
   WP_SYNC();
 #ifndef COOP_WRITE_PIPE
-#define COOP_WRITE_PIPE 0 /* 1: the next round's saved entry is requested one round ahead (measured: 1.05 -> 1.08 ms, not used) */
+#define COOP_WRITE_PIPE 0 /* 1: the next round's saved entry is requested one round ahead (slower when tuned before the H100 port, not used) */
 #endif
   U4 an, bn;
   an.x = an.y = an.z = an.w = bn.x = bn.y = bn.z = bn.w = 0u;

@@ -22,7 +22,7 @@
 #pragma once
 #include "ggr_encode.cuh"
 #ifndef COOP_WORD_COPY_MIN
-#define COOP_WORD_COPY_MIN 8u /* request emitter: 0.78 -> 0.75 ms against 12 */
+#define COOP_WORD_COPY_MIN 8u /* request emitter: faster than 12 when tuned before the H100 port */
 #endif
 #include "ggr_warp.cuh"
 
@@ -1209,7 +1209,7 @@ GGR_DEV bool ce_parse_item(SH& S, const CeLut& lut, const Tables& T, u32 root_ms
 // warp, 128 bytes per step.
 // ------------------------------------------------------------------------------------------------
 #ifndef CE_LONG_STR
-#define CE_LONG_STR 128u /* plain strings of at least this many bytes are copied by the whole warp (0.78 -> 0.75 ms against 96) */
+#define CE_LONG_STR 128u /* plain strings of at least this many bytes are copied by the whole warp (faster than 96 when tuned before the H100 port) */
 #endif
 #ifndef CE_LONG_MAX
 #define CE_LONG_MAX 32u
@@ -1217,7 +1217,7 @@ GGR_DEV bool ce_parse_item(SH& S, const CeLut& lut, const Tables& T, u32 root_ms
 #define CE_STAGE 8192u /* items with more wire bytes than this: per-thread emitter */
 #ifndef CE_STAGE_BUF
 /* the emitter's staging buffer; larger items (up to CE_STAGE and beyond) are written in place.  4864 + the lists = 5.3 KB per
-   warp = 10 blocks per SM instead of 6 with 8192 (configs[2]: wire items up to 4.6 KB; 1.11 -> 0.91 ms, profiles/README.md) */
+   warp = 10 blocks per SM instead of 6 with 8192 (configs[2]: wire items up to 4.6 KB) */
 #define CE_STAGE_BUF 4864u
 #endif
 struct
@@ -1235,7 +1235,7 @@ struct
 // one lane: bytes of node `i` into the staging buffer (long plain strings: payload left to the warp)
 // STAGED: byte position p of the item lands in the staging buffer (plain shared-memory stores); otherwise - items too
 // large to stage - at G[p], the destination itself shifted so that the same positions apply (two instances: a pointer
-// that may be either makes every store a generic one, 1.11 -> 1.67 ms on configs[2])
+// that may be either makes every store a generic one, much slower on configs[2] when tuned before the H100 port)
 // nd, off: node i and its offset, loaded by the caller (one round ahead: CE_EMIT_PIPE)
 template <bool STAGED>
 GGR_DEV void ce_emit_node(CoopEmit& E, u8* G, const u8* in, u32 end, const u8* ir, const u32* ioff, u32 i, u32 pad, const U4 nd, const u32 off) {

@@ -1185,7 +1185,7 @@ GGR_DEVN int put_map_field(W& w, const DecCtx& cx, u32 rpos, u32* rend, FieldD f
           if (str_keys) {
             // string keys: the first eight bytes (big-endian, zero-padded) and the length travel in the record, so that
             // a comparison of the sort is two register compares instead of a chain of loads from the wire (a 400-entry
-            // map costs about 7 000 comparisons per sort; measured on one lane: 83 ms for a 39 KB reply before)
+            // map costs about 7 000 comparisons per sort)
             const u32 kp = (u32)me.key, kl = (u32)(me.key >> 32);
             u64 P = 0;
             for (u32 j = 0; j < 8u; j++) P = (P << 8) | (j < kl ? (u64)cx.in[kp + j] : 0ull);

@@ -1,4 +1,4 @@
-// ggr_engine.cu - sm_100a kernels and the C ABI of include/ggrmcp_b200.h.
+// ggr_engine.cu - sm_90a kernels and the C ABI of include/ggrmcp_b200.h.
 //
 // Kernel plan (one item = one tools/call message, one thread per item, 128-thread blocks):
 //   request side : k_encode_parse  (pass A: JSON -> IR + exact size, block sums)
@@ -87,7 +87,7 @@ __global__ void __launch_bounds__(256) k_route(long long n, const u64* __restric
 }
 
 // Large items on the per-thread kernels: 32 unrelated state machines in one warp run their steps one after the other
-// (measured on the mixed replay: 1 320 replies of 16-39 KB take 502 ms together, the largest of them 83 ms alone), so an
+// (on the mixed replay a warp of large replies takes as long as all of them together), so an
 // item of at least `big_bytes` gets a warp of its own - slot 32 k of `spread` holds the item, the 31 entries behind it
 // none (the buffer is filled with 0xFF bytes before) - and the list-mode launches run over that list.  The list is
 // ordered by size class, largest first (five classes, each twice the one below): the warps of a launch are scheduled in
@@ -194,7 +194,7 @@ struct Slot {
 
 struct ggr_engine {
   int device = 0;
-  int sm_count = 148;
+  int sm_count = 132;
   int numa_node = -1;            // of the GPU's PCI function (sysfs), -1 unknown
   std::vector<int> node_cpus;    // CPUs of that node
   ggr::WireOrder order = ggr::ORDER_FIELD_NUMBER;
@@ -226,7 +226,7 @@ struct ggr_engine {
   int n_slots = 4;
   int64_t chunk_items = 8192;
   bool chunk_ramp = true;  // short chunks at both ends of a batch (GGR_CHUNK_RAMP=0: off)
-  // host-buffer entry points: the issuing threads either spin on the chunk events (lowest latency: +2.4 % end to end on one GPU)
+  // host-buffer entry points: the issuing threads either spin on the chunk events (lowest latency)
   // or sleep on them (cudaEventBlockingSync).  Spinning waiters of 8 engines are 16 busy threads: under a container CPU quota
   // they throttle every rank alike, so the default is to sleep when the quota leaves fewer than 4 CPUs per visible GPU
   // (usable_cpus(): affinity mask cut by cgroup cpu.max); GGR_BLOCKING_SYNC=0 / 1 decides by hand
@@ -424,7 +424,7 @@ int ggr_engine_create(const ggr_config* cfg, ggr_engine** out) {
   int dev = cfg ? cfg->device : 0;
   if (dev < 0 || dev >= ndev) return GGR_ERR_INVALID_ARGUMENT;
   if (cudaSetDevice(dev) != cudaSuccess) return GGR_ERR_NO_DEVICE;
-  // the library carries sm_100a code only: make sure the kernels are loadable here
+  // the library carries sm_90a code only: make sure the kernels are loadable here
   cudaFuncAttributes fa;
   if (cudaFuncGetAttributes(&fa, ggr_kernel_encode_parse()) != cudaSuccess) {
     cudaGetLastError();
@@ -433,7 +433,7 @@ int ggr_engine_create(const ggr_config* cfg, ggr_engine** out) {
   ggr_engine* e = new ggr_engine();
   e->device = dev;
   cudaDeviceGetAttribute(&e->sm_count, cudaDevAttrMultiProcessorCount, dev);
-  if (e->sm_count <= 0) e->sm_count = 148;
+  if (e->sm_count <= 0) e->sm_count = 132;
   find_numa(e);
   if (const char* nc = getenv("GGR_COOP")) e->use_coop = nc[0] != '0';
   if (const char* nc = getenv("GGR_COOP_ENC")) e->use_coop_enc = nc[0] != '0';
@@ -1046,7 +1046,7 @@ static bool slot_init(ggr_engine* e, Slot& sl) {
   return true;
 }
 
-// A large copy whose HOST address is not page aligned runs at 42.7 instead of 49.6 GB/s with both directions busy
+// A large copy whose HOST address is not page aligned runs slower with both directions busy
 // (scripts/pcie_align_probe.py; the device address does not matter).  Chunk boundaries are item boundaries and the output is
 // packed, so the host side of a chunk's payload is never aligned: the few bytes up to the next 4 KB boundary go first, the
 // rest starts on the boundary.
@@ -1165,7 +1165,7 @@ static int run_host(ggr_engine* e, const ggr_schema* s, bool encode, int64_t n, 
     };
     // A batch of several chunks starts and ends with short ones (a quarter, then half a chunk): the output link idles
     // until the first chunk's kernels are done and the input link idles while the last chunk drains, and both waits
-    // shrink with the chunk (profiles/README.md, host pipeline trace).
+    // shrink with the chunk (GGR_TRACE=1 shows the timeline).
     const bool ramp = e->chunk_ramp && n >= 4 * CH && CH >= 512;
     const int64_t tail0 = ramp ? n - (CH / 2 + CH / 4) : n, tail1 = ramp ? n - CH / 4 : n;
     int64_t i = 0;

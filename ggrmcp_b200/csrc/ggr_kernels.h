@@ -1,4 +1,4 @@
-// ggr_kernels.h - host-callable launchers of the sm_100a kernels (one translation unit per
+// ggr_kernels.h - host-callable launchers of the sm_90a kernels (one translation unit per
 // direction so they compile in parallel).
 #pragma once
 #include <cuda_runtime.h>
@@ -68,5 +68,5 @@ void ggr_launch_offsets(cudaStream_t st, unsigned nb, long long n, const uint32_
 void ggr_launch_wrap_write(cudaStream_t st, long long n, const uint8_t* text, const uint64_t* text_off, int32_t* status,
                            const uint8_t* ids, const uint64_t* ids_off, const uint32_t* size, uint8_t* out, uint64_t out_cap,
                            const uint64_t* out_off, int sm_count);
-const void* ggr_kernel_encode_parse();  // for cudaFuncGetAttributes (is the sm_100a image loadable?)
+const void* ggr_kernel_encode_parse();  // for cudaFuncGetAttributes (is the sm_90a image loadable?)
 int ggr_decode_max_rec();

@@ -118,8 +118,8 @@ k_encode_coop_emit(long long n, const u8* __restrict__ in, const u64* __restrict
   const u32 warp = threadIdx.x >> 5;
   const u64 a0 = in_off[0];
   const long long total = (long long)*list_n;  // the router's lock-step items
-  // fixed stride here: an item takes a few microseconds, tickets for 150 K of them in a millisecond
-  // run into the rate of atomics on one address (measured: 1.15 ms with the stride, 1.23 ms by ticket)
+  // fixed stride here: an item takes a few microseconds, and tickets for a whole batch of them in a millisecond
+  // would run into the rate of atomics on one address
   for (long long slot = (long long)blockIdx.x * CE_WARPS + warp; slot < total; slot += (long long)gridDim.x * CE_WARPS) {
     const long long item = (long long)list[slot];
     const u32 nw = nnodes[item];

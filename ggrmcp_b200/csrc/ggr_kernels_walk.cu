@@ -15,7 +15,7 @@
 #define CW_PLACE_BLOCKS 12
 #endif
 #ifndef CW_WALK_BLOCKS
-#define CW_WALK_BLOCKS 6 /* 80 registers, no spills: 1.71 ms against 1.78 with 7 blocks (72 registers, 264 bytes of spills) and 1.86 with 8 */
+#define CW_WALK_BLOCKS 6 /* 80 registers, no spills; 7 or 8 blocks per SM spilled when tuned before the H100 port */
 #endif
 
 __global__ void __launch_bounds__(CW_WARPS * 32, CW_TOK_BLOCKS)
@@ -83,8 +83,8 @@ k_encode_type(const u8* __restrict__ blob, u32 n_msgs, const i32* __restrict__ m
   const u64 a0 = in_off[0];
   u32* ticket = const_cast<u32*>(list_n) + 2;  // +1 the tokenizer, +3 the place kernel
   // two tickets in flight (the draw's latency stays off the path).  A bulk L2 prefetch of the next item's index, records
-  // and text (cp.async.bulk.prefetch.L2) was measured here and cost 4 %: the index was written by the two kernels in
-  // front of this one and is L2-resident already (profiles/README.md)
+  // and text (cp.async.bulk.prefetch.L2) cost more than it saved here when tuned before the H100 port: the index was written by the two kernels in
+  // front of this one and is L2-resident already
   u32 drawn = wp_ticket_draw(ticket);
   long long slot = wp_ticket_take(drawn);
   drawn = wp_ticket_draw(ticket);

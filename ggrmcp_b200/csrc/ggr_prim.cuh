@@ -8,7 +8,7 @@
 //
 // The same code compiles as plain C++ for the host simulation used by the CPU-side tests
 // (tests/hostsim): there is no GPU in the build container, so kernel logic is debugged there and
-// only confirmed on the B200.  The shipped library contains the __device__ build only.
+// only confirmed on the H100.  The shipped library contains the __device__ build only.
 #pragma once
 #include <stdint.h>
 #include <string.h>
@@ -24,7 +24,7 @@
 #endif
 
 // Warp convergence for the one-item-per-thread walkers.  A message parser is a data-dependent state
-// machine; left alone, the 32 lanes of a warp drift apart for good (ncu: 1.7 active threads per
+// machine; left alone, the 32 lanes of a warp drift apart for good (few active threads per
 // instruction).  Every hot loop therefore runs as
 //     while (ggr_any(mask, !done)) { if (!done) { one bounded step; } }
 // so that all lanes of `mask` meet again at the vote after every step.

@@ -6,8 +6,7 @@
 // reference does here is protojson.Unmarshal into a dynamicpb message followed by proto.Marshal's size
 // pass (/root/reference/pkg/grpc/reflection.go:351-357,373).
 //
-// Three small kernels (each one's hot loop fits the instruction caches; the fused form measured 11.4 K warp
-// instructions per item at 43 % issue with 5 no-instruction stalls per issue, profiles/README.md):
+// Three small kernels (each one's hot loop fits the instruction caches, which the fused form's did not):
 //   k_encode_tok3  : T1 - bit-mask tokenizer as in ggr_coop_enc.cuh, but colons and commas are consumed
 //                    here: which token may follow which is checked on bit masks (carry-propagating adds
 //                    find every token's predecessor), the surviving tokens - brackets, strings, scalars -
@@ -538,7 +537,7 @@ enum {
 };
 
 #ifndef CW_TYPE_PRE
-#define CW_TYPE_PRE 0 /* 1: token, key and string quote entries of every record fetched with full lanes before the level pass (measured: 1.52 -> 1.63 ms, not used) */
+#define CW_TYPE_PRE 0 /* 1: token, key and string quote entries of every record fetched with full lanes before the level pass (slower when tuned before the H100 port, not used) */
 #endif
 template <int MN>
 struct CoopWalkT {

@@ -1,6 +1,6 @@
 // ggr_warp.cuh - warp collectives for the lock-step (one warp per item) kernels.
 //
-// Device build: thin wrappers over the sm_100a warp intrinsics, full mask, all 32 lanes call
+// Device build: thin wrappers over the sm_90a warp intrinsics, full mask, all 32 lanes call
 // together.  Host build (tests/hostsim only): the same source runs as 32 cooperative fibers, one
 // per lane; every collective is a rendezvous through an exchange array, and every rendezvous
 // carries the source line it was called from so that lanes that reach different collectives
@@ -272,8 +272,8 @@ GGR_DEV void coop_copy_words(const u8* in, u32 src, u8* d, u32 len) {
 }
 
 // One lane: len bytes of read-only data at s to d, four at a time - head bytes until d is word aligned, then aligned
-// word loads of the source brought into place by a funnel shift and one word store each (the byte loop was 28 % of
-// the reply write kernel's instructions and 57 % of the request emitter's, profiles/README.md).  A source word is only loaded
+// word loads of the source brought into place by a funnel shift and one word store each (a byte loop was a large share of
+// the reply write kernel's and the request emitter's instructions).  A source word is only loaded
 // when it holds at least one byte of [s, s + len).
 #ifndef COOP_WORD_COPY_MIN
 #define COOP_WORD_COPY_MIN 12u /* shorter runs: byte by byte */

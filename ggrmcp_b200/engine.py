@@ -134,7 +134,7 @@ class Engine:
         h = C.c_void_p()
         rc = L.ggr_engine_create(C.byref(cfg), C.byref(h))
         if rc != 0:
-            raise EngineError("ggr_engine_create failed with %d (no CUDA device / sm_100a kernels not loadable); "
+            raise EngineError("ggr_engine_create failed with %d (no CUDA device / sm_90a kernels not loadable); "
                               "this engine has no CPU path" % rc)
         self.h = h
         self.device = device

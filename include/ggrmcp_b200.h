@@ -1,5 +1,5 @@
 /*
- * ggrmcp_b200.h - C ABI of the B200 transcoding engine for ggRMCP's tools/call hot path.
+ * ggrmcp_b200.h - C ABI of the GPU transcoding engine for ggRMCP's tools/call hot path.
  *
  * Drop-in boundary (SURVEY.md section 8b).  The reference has no FFI; every entry point below
  * names the reference interface it stands in for, so that a cgo shim (INTEGRATION.md) can sit
@@ -20,7 +20,7 @@
  *
  * Plain C types only, no callbacks, no torch types.  All buffers are borrowed for the duration of
  * the call.  One bad item never fails the batch: every item gets its own status.
- * There is no CPU fallback: every transcode runs in the sm_100a kernels; without a CUDA device
+ * There is no CPU fallback: every transcode runs in the sm_90a kernels; without a CUDA device
  * ggr_engine_create fails with GGR_ERR_NO_DEVICE.
  */
 #ifndef GGRMCP_B200_H_
@@ -109,7 +109,7 @@ uint64_t ggr_launch_count(const ggr_engine* e);  /* kernels launched by this eng
  * ggr_host_alloc returns page-locked memory whose pages sit on the NUMA node the engine's GPU hangs off
  * (the calling thread is bound to that node's CPUs while the pages are allocated and touched, then put
  * back), so that the copies of the chunked pipeline do not cross the socket interconnect: with 8 GPUs on
- * two sockets that is the difference between 18 and 36 GB/s per GPU (profiles/README.md).  A Go shim
+ * two sockets a remote node can halve the copy rate per GPU.  A Go shim
  * allocates its arenas here instead of in the Go heap.  ggr_device_numa_node: -1 when the platform does
  * not say.  ggr_bind_thread_to_device binds the calling thread (a per-GPU batching thread) to the same CPUs.
  */

@@ -1,5 +1,5 @@
-"""profiles/sass_sizes_r2.txt: .text bytes, registers and TMA-class instructions (UBLKCP bulk copy, UBLKPF bulk prefetch,
-SYNCS mbarrier) of every kernel in the shipped library.   usage: python scripts/sass_report.py > profiles/sass_sizes_r2.txt"""
+""".text bytes, registers and TMA-class instructions (UBLKCP bulk copy, UBLKPF bulk prefetch, SYNCS mbarrier) of every
+kernel in the shipped library.   usage: python scripts/sass_report.py"""
 import collections
 import os
 import re
@@ -37,7 +37,7 @@ for ln in res.splitlines():
         regs[fn] = (int(m.group(1)), int(m.group(2)))
 dem = subprocess.run(["c++filt"] + list(sizes), capture_output=True, text=True).stdout.splitlines()
 names = dict(zip(sizes, dem))
-print("# kernels of ggrmcp_b200/libggrmcp_b200.so (sm_100a): .text bytes, registers, static shared memory, bulk / TMA-class SASS")
+print("# kernels of ggrmcp_b200/libggrmcp_b200.so (sm_90a): .text bytes, registers, static shared memory, bulk / TMA-class SASS")
 print("%-9s %5s %7s  %-22s %s" % (".text", "regs", "smem", "UBLKCP/UBLKPF/SYNCS", "kernel"))
 for k, v in sorted(sizes.items(), key=lambda kv: -kv[1]):
     r = regs.get(k, (0, 0))

@@ -10,7 +10,7 @@ for p in (ROOT, os.path.join(ROOT, "tests")):
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100; select with -m gpu)")
 
 
 @pytest.fixture(scope="session")
@@ -68,15 +68,8 @@ def engine(request):
                 os.environ.pop(k, None)
             else:
                 os.environ[k] = v
-    e.path_name = request.param
     yield e
     e.close()
-
-
-def heavy(engine, paths=("default", "size_routing")):
-    """full-size tests run on the two product paths only (the other engine paths repeat the small corpora)"""
-    if getattr(engine, "path_name", "default") not in paths:
-        pytest.skip("full-size test: runs on the %s path(s)" % "/".join(paths))
 
 
 @pytest.fixture(scope="session")

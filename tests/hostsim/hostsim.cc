@@ -3,7 +3,7 @@
 // The build container has no GPU.  The per-message device functions in ggrmcp_b200/csrc/*.cuh are
 // written against a tiny load/store shim (ggr_prim.cuh) so that exactly the same parser / emitter
 // code can be compiled here with g++ and run one "thread" at a time against the oracle.  This
-// library is never loaded by the product; the shipped .so contains only the sm_100a build and
+// library is never loaded by the product; the shipped .so contains only the sm_90a build and
 // fails loudly without a CUDA device.
 #include <cstdlib>
 #include <cstring>

@@ -1,4 +1,4 @@
-"""GPU parity tests: the sm_100a kernels, driven through the C ABI (ggr_encode_batch /
+"""GPU parity tests: the sm_90a kernels, driven through the C ABI (ggr_encode_batch /
 ggr_decode_batch), against the CPU oracle on the same inputs.  Bit-exact for every item the
 oracle accepts; equal status category for every item it rejects."""
 import random
@@ -7,7 +7,6 @@ import numpy as np
 import pytest
 
 import cases
-from conftest import heavy
 
 pytestmark = pytest.mark.gpu
 
@@ -202,7 +201,6 @@ def test_empty_and_ragged_batches(engine, schema, oracle):
 
 def test_full_size_properties(engine, schema, oracle):
     """BASELINE.json config sizes: round trip wire -> JSON -> wire and sampled oracle parity."""
-    heavy(engine, ('default', 'size_routing', 'poisoned'))
     import benchgen
     n = 65536
     wl = benchgen.nested(n, schema.message)
@@ -240,7 +238,6 @@ def oracle_index(oracle, schema, engine_idx):
 
 
 def test_flat_and_blob_configs(engine, schema, oracle):
-    heavy(engine)
     import benchgen
     wl = benchgen.flat(65536, schema.message)
     wire, woff, st = engine.encode_batch(schema, wl.req_msg, wl.req_json, wl.req_off)
@@ -266,7 +263,6 @@ def test_flat_and_blob_configs(engine, schema, oracle):
 def test_request_and_reply_batches_in_flight_together(engine, schema, oracle):
     """the host entry points take one batch per direction concurrently (bench.py's end-to-end run does
     exactly this from two threads): results must be those of the calls made one after the other"""
-    heavy(engine, ('default', 'small_chunks', 'ramped_chunks'))
     import threading
     import benchgen
     n = 20000
@@ -395,7 +391,6 @@ def test_go_legacy_field_order(schema, oracle, fds_bytes):
 def test_small_output_capacity(engine, schema, oracle):
     """GGR_ERR_NO_SPACE: out_off[n] comes back as the capacity that would do, for one chunk and for many, in
     both directions and with result wrapping; the retry with that capacity gives the full result"""
-    heavy(engine, ('default', 'small_chunks', 'ramped_chunks'))
     import ctypes as C
     import benchgen
     from ggrmcp_b200 import engine as E
@@ -473,7 +468,6 @@ _mixed_cache = {}
 
 def test_mixed_replay(engine, schema, oracle):
     """configs[4]: 100 000 calls over 32 methods with Zipf-distributed sizes, every item against the oracle"""
-    heavy(engine, ('default', 'size_routing', 'per_thread', 'poisoned'))
     import os
     import benchgen
     if not _mixed_cache:

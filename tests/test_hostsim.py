@@ -495,7 +495,7 @@ def test_mixed_replay_shapes(oracle, hsim):
         rc, oj, _ = oracle.decode(pn, w)
         st, ej = hsim.decode(pn, w, 0, i % 16, (i * 7) % 16)
         assert rc == 0 and st == 0 and ej == oj, (pn, w.hex()[:300])
-    assert walked > 150  # floats, bytes, quoted numbers, timestamps: the fused kernel (profiles/README.md)
+    assert walked > 150  # floats, bytes, quoted numbers, timestamps: the fused kernel
     # request side, large items: the three walker tiers (the third: up to 8192 values) against the oracle
     huge = 0
     for i in range(wl.n):
