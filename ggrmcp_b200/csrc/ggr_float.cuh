@@ -250,18 +250,23 @@ GGR_DEVN void put_float_go(W& w, u64 bits, bool is32) {
 // decimal -> binary, correctly rounded
 // ------------------------------------------------------------------------------------------------
 #define GGR_BIG_WORDS 40
-struct Big {
-  u32 w[GGR_BIG_WORDS];
+// little-endian u32 words; NW words of capacity
+template <int NW>
+struct BigN {
+  u32 w[NW];
   int n;  // words in use (no leading zero words), 0 for zero
 };
-GGR_DEV void big_set64(Big& b, u64 v) {
+using Big = BigN<GGR_BIG_WORDS>;
+template <int NW>
+GGR_DEV void big_set64(BigN<NW>& b, u64 v) {
   b.n = 0;
   if (v) {
     b.w[b.n++] = (u32)v;
     if (v >> 32) b.w[b.n++] = (u32)(v >> 32);
   }
 }
-GGR_DEV bool big_mul_small(Big& b, u32 f, u32 add) {  // b = b*f + add; false on capacity overflow
+template <int NW>
+GGR_DEV bool big_mul_small(BigN<NW>& b, u32 f, u32 add) {  // b = b*f + add; false on capacity overflow
   u64 carry = add;
   for (int i = 0; i < b.n; i++) {
     u64 t = (u64)b.w[i] * f + carry;
@@ -269,12 +274,13 @@ GGR_DEV bool big_mul_small(Big& b, u32 f, u32 add) {  // b = b*f + add; false on
     carry = t >> 32;
   }
   if (carry) {
-    if (b.n >= GGR_BIG_WORDS) return false;
+    if (b.n >= NW) return false;
     b.w[b.n++] = (u32)carry;
   }
   return true;
 }
-GGR_DEV bool big_mul_pow5(Big& b, u32 k) {
+template <int NW>
+GGR_DEV bool big_mul_pow5(BigN<NW>& b, u32 k) {
   while (k >= 13) {
     if (!big_mul_small(b, 1220703125u, 0)) return false;
     k -= 13;
@@ -283,19 +289,23 @@ GGR_DEV bool big_mul_pow5(Big& b, u32 k) {
   for (u32 i = 0; i < k; i++) f *= 5;
   return f == 1 ? true : big_mul_small(b, f, 0);
 }
-GGR_DEV int big_bitlen(const Big& b) {
+template <int NW>
+GGR_DEV int big_bitlen(const BigN<NW>& b) {
   if (b.n == 0) return 0;
   u32 top = b.w[b.n - 1];
   return 32 * (b.n - 1) + (32 - (ggr_clz64((u64)top) - 32));
 }
-GGR_DEV u32 big_bit(const Big& b, int i) { return (i < 0 || (i >> 5) >= b.n) ? 0u : (b.w[i >> 5] >> (i & 31)) & 1u; }
-GGR_DEV int big_cmp(const Big& a, const Big& b) {
+template <int NW>
+GGR_DEV u32 big_bit(const BigN<NW>& b, int i) { return (i < 0 || (i >> 5) >= b.n) ? 0u : (b.w[i >> 5] >> (i & 31)) & 1u; }
+template <int NW>
+GGR_DEV int big_cmp(const BigN<NW>& a, const BigN<NW>& b) {
   if (a.n != b.n) return a.n < b.n ? -1 : 1;
   for (int i = a.n - 1; i >= 0; i--)
     if (a.w[i] != b.w[i]) return a.w[i] < b.w[i] ? -1 : 1;
   return 0;
 }
-GGR_DEV void big_sub(Big& a, const Big& b) {  // a -= b, a >= b
+template <int NW>
+GGR_DEV void big_sub(BigN<NW>& a, const BigN<NW>& b) {  // a -= b, a >= b
   u64 borrow = 0;
   for (int i = 0; i < a.n; i++) {
     u64 t = (u64)a.w[i] - (i < b.n ? b.w[i] : 0u) - borrow;
@@ -304,7 +314,8 @@ GGR_DEV void big_sub(Big& a, const Big& b) {  // a -= b, a >= b
   }
   while (a.n > 0 && a.w[a.n - 1] == 0) a.n--;
 }
-GGR_DEV bool big_shl1_add(Big& a, u32 bit) {  // a = a*2 + bit
+template <int NW>
+GGR_DEV bool big_shl1_add(BigN<NW>& a, u32 bit) {  // a = a*2 + bit
   u32 carry = bit;
   for (int i = 0; i < a.n; i++) {
     u32 t = a.w[i];
@@ -312,9 +323,24 @@ GGR_DEV bool big_shl1_add(Big& a, u32 bit) {  // a = a*2 + bit
     carry = t >> 31;
   }
   if (carry) {
-    if (a.n >= GGR_BIG_WORDS) return false;
+    if (a.n >= NW) return false;
     a.w[a.n++] = carry;
   }
+  return true;
+}
+template <int NW>
+GGR_DEV bool big_shl(BigN<NW>& a, u32 s) {  // a <<= s; false on capacity overflow
+  if (a.n == 0) return true;
+  const int ws = (int)(s >> 5), bs = (int)(s & 31u);
+  const int n = a.n + ws + (bs != 0 && (a.w[a.n - 1] >> (32 - bs)) != 0 ? 1 : 0);
+  if (n > NW) return false;
+  for (int i = n - 1; i >= 0; i--) {
+    const int j = i - ws;  // source word
+    const u32 hi = j >= 0 && j < a.n ? a.w[j] : 0u;
+    const u32 lo = j - 1 >= 0 && j - 1 < a.n ? a.w[j - 1] : 0u;
+    a.w[i] = bs ? (hi << bs) | (lo >> (32 - bs)) : hi;
+  }
+  a.n = n;
   return true;
 }
 
@@ -447,6 +473,76 @@ GGR_DEV u32 fl_float_bits(float f) {
   return u;
 }
 
+// Long literals: the exact decision when the first 40 significant digits leave the rounding open, i.e. the
+// value lies within about 10^-39 (relative) of the halfway point H = (2m+1) * 2^(e-1) between lo = m * 2^e and
+// the next float up.  Like Go's strconv it reads at most 800 significant digits N, value = N * 10^k, plus
+// whether a nonzero digit follows.  That is exact: a halfway point has at most 767 significant digits, so it
+// never lies strictly between N * 10^k and (N+1) * 10^k.  Both sides of N * 10^k <=> (2m+1) * 2^(e-1) are
+// scaled to integers; near a halfway point neither exceeds 2^2670 (binary64: N < 10^800, or 2^55 * 5^1124 with
+// k >= -1124), which GGR_XBIG_WORDS covers with room to spare.  Kept out of float_from_token's frame: only
+// literals that reach it pay for the large integers.  `it` is at the token's first character.  Returns the
+// correctly rounded bits without the sign; false on overflow (ParseFloat's range error).
+#define GGR_XBIG_WORDS 88
+template <class It>
+GGR_DEVN bool fl_decide_long(It it, i32 exp10, u64 lo, bool is32, u64* out) {
+  using XBig = BigN<GGR_XBIG_WORDS>;
+  XBig A, B;
+  A.n = 0;
+  if (it.get() == '-') it.adv();
+  u32 kept = 0, acc = 0, nacc = 0, pow = 1;
+  i64 k = exp10;
+  bool more = false, in_frac = false;
+  for (;;) {
+    const u32 c = it.get();
+    if (it.eof()) break;
+    if (c == '.') {
+      in_frac = true;
+      it.adv();
+      continue;
+    }
+    if (!(c - '0' < 10u)) break;
+    const u32 dgt = c - '0';
+    if (in_frac) k--;
+    if (kept == 0 && dgt == 0) {  // leading zeros
+      it.adv();
+      continue;
+    }
+    if (kept < 800) {
+      acc = acc * 10 + dgt;
+      pow *= 10;
+      kept++;
+      if (++nacc == 9) {
+        if (!big_mul_small(A, pow, acc)) return false;
+        acc = nacc = 0;
+        pow = 1;
+      }
+    } else {
+      k++;
+      if (dgt != 0) more = true;
+    }
+    it.adv();
+  }
+  if (nacc && !big_mul_small(A, pow, acc)) return false;
+  const int mbits = is32 ? 23 : 52, bias = is32 ? 127 : 1023;
+  const u32 be = (u32)(lo >> mbits);
+  u64 m = lo & ((1ull << mbits) - 1ull);
+  i32 e = 1 - bias - mbits;
+  if (be != 0) {
+    m |= 1ull << mbits;
+    e = (i32)be - bias - mbits;
+  }
+  big_set64(B, 2 * m + 1);
+  const i64 p = (i64)e - 1;  // H = B * 2^p
+  if (k >= 0 ? !big_mul_pow5(A, (u32)k) : !big_mul_pow5(B, (u32)-k)) return false;
+  if (k - p >= 0 ? !big_shl(A, (u32)(k - p)) : !big_shl(B, (u32)(p - k))) return false;
+  int c = big_cmp(A, B);
+  if (c == 0 && more) c = 1;
+  const u64 r = lo + ((c > 0 || (c == 0 && (m & 1ull))) ? 1u : 0u);  // the carry runs into the exponent field
+  if ((r >> mbits) >= (is32 ? 255u : 2047u)) return false;
+  *out = r;
+  return true;
+}
+
 template <class It>
 GGR_DEVN bool float_from_token(It again, const NumTok& t, bool is32, u64* bits) {
   const u64 sign = t.neg ? (is32 ? 0x80000000ull : 0x8000000000000000ull) : 0ull;
@@ -483,7 +579,9 @@ GGR_DEVN bool float_from_token(It again, const NumTok& t, bool is32, u64* bits) 
     big_set64(D, t.m);
   } else {
     // more significant digits than fit 64 bits: re-read them into a big integer (the first 40
-    // significant digits exactly, the rest as a sticky bit)
+    // significant digits exactly, the rest as a sticky bit; fl_decide_long reads them again if needed)
+    Rd from_rd;
+    const It from = it_fork(again, &from_rd);
     D.n = 0;
     u32 c = again.get();
     if (c == '-') again.adv();
@@ -521,6 +619,19 @@ GGR_DEVN bool float_from_token(It again, const NumTok& t, bool is32, u64* bits) 
     if (kk > 100000) kk = 100000;
     if (kk < -100000) kk = -100000;
     k = (i32)kk;
+    if (sticky) {
+      // nonzero digits were dropped: D * 10^k < value < (D+1) * 10^k.  Rounding is monotone, so when
+      // both bounds round to the same float that is the answer; otherwise the digits decide.
+      Big D1;
+      D1.n = D.n;
+      for (int i = 0; i < D.n; i++) D1.w[i] = D.w[i];
+      big_mul_small(D1, 1, 1);  // D has at most 40 digits: no capacity overflow
+      u64 lo, hi;
+      if (!fl_from_big(D, k, true, is32, &lo)) return false;  // the lower bound overflows: so does the value
+      if ((!fl_from_big(D1, k, false, is32, &hi) || hi != lo) && !fl_decide_long(from, t.exp, lo, is32, &lo)) return false;
+      *bits = lo | sign;
+      return true;
+    }
   }
   u64 out;
   if (!fl_from_big(D, k, sticky, is32, &out)) return false;

@@ -210,6 +210,14 @@ struct RawIter {
   GGR_DEV u32 get() const { return r->get(); }
   GGR_DEV void adv() { r->skip(1); }
 };
+// an independent iterator at the same position, for a second pass over a token (a RawIter shares its
+// reader, so its copy reads from `store`)
+GGR_DEV StrIter it_fork(const StrIter& it, Rd*) { return it; }
+GGR_DEV RawIter it_fork(const RawIter& it, Rd* store) {
+  *store = *it.r;
+  RawIter c = {store};
+  return c;
+}
 
 // ------------------------------------------------------------------------------------------
 // Number tokens.  m * 10^k is the exact value when the token is an integer (see DESIGN.md):

@@ -126,6 +126,13 @@ ENCODE_EDGE = [
     (A, b'{"f_double":1e99999999999}', None), (A, b'{"f_int32":0e99999999999}', None), (A, b'{"f_uint64":"0e-99999999999"}', None),
     (A, b'{"f_int64":0e100000000,"f_sint32":0e-100000000}', None), (A, b'{"f_int64":0e100000001}', None),
     (A, b'{"r_double":[0e100000001,5e-100000001,0.0e00000000000000000000001]}', None),
+    # halfway points written exactly, and followed by a nonzero digit far behind the 40th significant one: 1 and the
+    # next double up, 0 and the smallest float32 / double subnormal, DBL_MAX and 2^1024 (out of range above the tie)
+    (A, b'{"f_double":1.00000000000000011102230246251565404236316680908203125}', None),
+    (A, b'{"f_double":1.000000000000000111022302462515654042363166809082031250001}', None),
+    (A, b'{"f_float":0.%s0001}' % str(5 ** 150).rjust(150, "0").encode(), None),
+    (A, b'{"f_double":0.%s0001}' % str(5 ** 1075).rjust(1075, "0").encode(), None),
+    (A, b'{"f_double":%d.0001,"f_int32":1}' % ((2 ** 54 - 1) << 970), None), (A, b'{"f_double":-%d}' % ((2 ** 54 - 1) << 970), None),
 ]
 
 DECODE_EDGE_HEX = [

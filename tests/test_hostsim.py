@@ -569,3 +569,67 @@ def test_byte_run_copies(hsim):
     L = hostsim.lib()
     L.hs_copy_selftest.argtypes = [C.c_uint32]
     assert L.hs_copy_selftest(300) == 0
+
+
+# ---- float and double text conversion against the exact reference (numref) ------------------------------------
+_num_cache = {}
+
+
+def _num_corpus():
+    import numcorpus as NC
+    if not _num_cache:
+        lits = NC.request_literals()
+        _num_cache["req"] = NC.request_items(lits)
+        _num_cache["bodies"] = NC.body_items(lits)
+        _num_cache["rep"] = NC.reply_items(NC.reply_bits(64, n_random=30000), NC.reply_bits(32, stride=65521))
+    return _num_cache
+
+
+def _wire_matches(st, out, want):
+    import numref
+    return st != 0 if want == numref.RANGE else (st == 0 and out == want)
+
+
+def test_numbers_request_per_thread(hsim):
+    """halfway points written exactly, just above and just below with the deciding digit up to 1500 significant
+    digits in, fast-path edges, float32 double-rounding traps: the per-thread parser rounds like strconv.ParseFloat"""
+    bad = [(n, js[:120]) for i, (n, js, want) in enumerate(_num_corpus()["req"]) if not _wire_matches(*hsim.encode(n, js, i % 16, (i * 5) % 16), want)]
+    assert not bad, (len(bad), bad[:5])
+
+
+@pytest.mark.parametrize("tier", [0, 1])
+def test_numbers_request_lockstep(hsim, tier):
+    """the lock-step parser either leaves an item to the per-thread parser (200) or gives the exact bytes"""
+    handled = 0
+    for i, (n, js, want) in enumerate(_num_corpus()["req"]):
+        rc, out = hsim.encode_coop(n, js, i % 16, (i * 5) % 16, tier)
+        if rc == 200:
+            continue
+        assert _wire_matches(rc, out, want), (n, js[:120], rc)
+        handled += 1
+    assert handled > len(_num_corpus()["req"]) // 2
+
+
+def test_numbers_request_envelope(hsim):
+    """tools/call bodies: a bare literal takes json.Marshal's float64 round trip, a quoted one reaches the field as
+    written; every body is taken, a literal out of float64 range is refused"""
+    import numref
+    for i, (body, want) in enumerate(_num_corpus()["bodies"]):
+        rc, wire, method, idt = hsim.request_coop(body, i % 16, (i * 3) % 16, i & 1)
+        if want == numref.RANGE:
+            assert rc != 0, body[:200]
+        else:
+            assert rc == 0 and wire == want, (body[:200], rc, wire.hex())
+
+
+def test_numbers_reply(hsim):
+    """shortest round-trip text of doubles and floats in packed runs, unpacked occurrences, singular fields, map
+    values and wrappers; the lock-step reply side gives the same text or leaves the item (200)"""
+    taken = 0
+    for i, (n, w, want) in enumerate(_num_corpus()["rep"]):
+        rc, out = hsim.decode(n, w, 0, i % 16, (i * 5) % 16)
+        assert rc == 0 and out == want, (n, w.hex()[:80], out[:200], want[:200])
+        rc, out = hsim.decode_coop(n, w, 0, i % 16, (i * 5) % 16)
+        assert rc == 200 or (rc == 0 and out == want), (n, w.hex()[:80], rc, out[:200], want[:200])
+        taken += rc == 0
+    assert taken > 1000

@@ -9,6 +9,7 @@ import struct
 import pytest
 
 import cases
+import numref
 import orc
 import pbgen
 
@@ -103,31 +104,6 @@ def test_error_envelopes(oracle):
     assert r["kind"] == 2 and b"tool nope_tool not found" in r["resp"]
 
 
-def go_style(v):
-    """Python shortest repr -> the ES6-style text encoding/json and protojson print"""
-    import decimal
-    if v == 0:
-        return "-0" if math.copysign(1, v) < 0 else "0"
-    d = decimal.Decimal(repr(abs(v)))
-    _, digits, exp = d.as_tuple()
-    ds = "".join(map(str, digits))
-    stripped = ds.rstrip("0") or "0"
-    exp += len(ds) - len(stripped)
-    ds = stripped
-    x = len(ds) + exp
-    neg = "-" if v < 0 else ""
-    a = abs(v)
-    if a < 1e-6 or a >= 1e21:
-        e = x - 1
-        m = ds[0] + ("." + ds[1:] if len(ds) > 1 else "")
-        return neg + m + ("e-%d" % (-e) if e < 0 else "e+%02d" % e)
-    if x <= 0:
-        return neg + "0." + "0" * (-x) + ds
-    if len(ds) <= x:
-        return neg + ds + "0" * (x - len(ds))
-    return neg + ds[:x] + "." + ds[x:]
-
-
 def test_float_format_matches_shortest_repr():
     rng = random.Random(7)
     for i in range(20000):
@@ -139,12 +115,44 @@ def test_float_format_matches_shortest_repr():
             v = float(rng.randint(-10 ** rng.randint(1, 18), 10 ** rng.randint(1, 18)))
         if v != v or math.isinf(v):
             continue
-        assert orc.format_float(v) == go_style(v), repr(v)
+        assert orc.format_float(v) == numref.format_float(v), repr(v)
     for v, s in [(1.0, "1"), (1e21, "1e+21"), (1e-7, "1e-7"), (1e-6, "0.000001"), (123456789012345680000.0, "123456789012345680000"),
                  (5e-324, "5e-324"), (-0.0, "-0")]:
         assert orc.format_float(v) == s
     assert orc.format_float(3.4028234663852886e38, 32) == "3.4028235e+38"
     assert orc.format_float(0.10000000149011612, 32) == "0.1"
+
+
+def test_float32_format_matches_numpy():
+    """float32 printing: the oracle's shortest digits equal numpy's shortest float32 on a strided sweep of all bit
+    patterns (with both layouts and their switch points), through numref's layout"""
+    import numpy as np
+    bits = np.arange(0, 1 << 32, 21011, dtype=np.uint64).astype(np.uint32)
+    bits = np.concatenate([bits, np.array([numref.parse(t, 32) + d for t in ("1e-6", "1e21") for d in (-1, 0, 1)], np.uint32)])
+    vals = bits.view(np.float32)
+    n = 0
+    for b, v in zip(bits.tolist(), vals.tolist()):
+        if v != v or math.isinf(v):
+            continue
+        assert orc.format_float(v, 32) == numref.format(b, 32), hex(b)
+        n += 1
+    assert n > 200000
+
+
+def test_number_corpus_matches_numref(oracle):
+    """the oracle rounds like strconv.ParseFloat and prints like strconv.AppendFloat on the number corpus: request
+    literals in every float position, tools/call bodies, and a reply sample"""
+    import numcorpus as NC
+    lits = NC.request_literals()
+    for n, js, want in NC.request_items(lits):
+        rc, out, _ = oracle.encode(n, js)
+        assert (rc != 0) if want == numref.RANGE else (rc == 0 and out == want), (n, js[:120], rc)
+    for body, want in NC.body_items(lits):
+        r = oracle.request(body)
+        assert (r["kind"] != 0) if want == numref.RANGE else (r["kind"] == 0 and r["wire"] == want), body[:200]
+    for n, w, want in NC.reply_items(NC.reply_bits(64, n_random=20000), NC.reply_bits(32, stride=99991)):
+        rc, out, _ = oracle.decode(n, w)
+        assert rc == 0 and out == want, (n, w.hex()[:80], out[:200], want[:200])
 
 
 def _json_equal(a, b):
