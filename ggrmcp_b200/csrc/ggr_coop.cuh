@@ -19,9 +19,6 @@
 // them on 32 fibers).
 #pragma once
 #include "ggr_decode.cuh"
-#ifndef COOP_WORD_COPY_MIN
-#define COOP_WORD_COPY_MIN 24u /* reply write kernel: faster than 12 when tuned before the H100 port */
-#endif
 #include "ggr_warp.cuh"
 
 // why the lock-step tier left an item: recorded by the host simulation only (tests/hostsim: hs_coop_why = source line)
@@ -37,9 +34,7 @@ extern int g_coop_why;
 // 24 warps per SM), the full 320 in the second tier, which takes the few items the first leaves because of the table
 // (one such item on the per-thread kernels costs half a millisecond of one lane: the tail of the whole batch).
 #define GGR_COOP_TAB_ENTRIES 320
-#ifndef GGR_COOP_ENTRIES
 #define GGR_COOP_ENTRIES 224
-#endif
 #define GGR_COOP_DEPTH 24
 #define GGR_COOP_MAX_WIRE 4096u  /* larger items: no plain-text masks, strings are classified one by one */
 #define GGR_MODE_COOP 2u
@@ -70,18 +65,8 @@ struct CoopEnt {            // 32 bytes: saved between the passes as two 16-byte
 #define GGR_COOP_ROOT 0xFFFFu
 #define CE_CLASS(e) (((e).flags >> CF_CLASS_SHIFT) & 0xFu)
 
-#ifndef GGR_COOP_LONG
 #define GGR_COOP_LONG 96u /* plain strings of at least this many bytes are copied by the whole warp */
-#endif
-#ifndef GGR_COOP_LONG_MAX
 #define GGR_COOP_LONG_MAX 32u
-#endif
-#ifndef COOP_WIN_CACHE
-#define COOP_WIN_CACHE 0 /* 1: the scan keeps two 16-byte chunks in registers (slower when tuned before the H100 port, not used) */
-#endif
-#ifndef COOP_COLD_LEAF
-#define COOP_COLD_LEAF 0 /* 1: float / timestamp sizing as a call (slower when tuned before the H100 port, not used) */
-#endif
 #define GGR_COOP_DIRTY_MAX 64u
 template <int NE>
 struct CoopSharedT {
@@ -169,33 +154,6 @@ GGR_DEV bool coop_wire_zero(const u8* b, u32 pos, u32 lim, u32 wt, bool* ok) {
 
 // coop_window / coop_header (a field header out of one 8-byte window): ggr_decode.cuh, shared with the slow walk
 
-// The scan's window with a memory: the 16-byte chunk that holds `pos` and the one behind it stay in registers, so a
-// run of small fields (a handful of bytes each: the usual reply) costs one round trip to the L2 per chunk instead of
-// one per field.  Returns what coop_window returns: the 8 bytes at pos, bytes from end_al on read as zero.
-struct CoopWinCache {
-  u32 base;  // position of chunk a (a multiple of 16), 0xFFFFFFFF: nothing held
-  U4 a, b;
-  GGR_DEV u64 get(const u8* in, u32 pos, u32 end_al) {
-    const u32 c = pos & ~15u;
-    if (c != base) {
-      base = c;
-      a = ggr_ld16(in + c);
-      if (c + 16u < end_al) b = ggr_ld16(in + c + 16u);
-      else b.x = b.y = b.z = b.w = 0u;
-    }
-    const u32 k = (pos >> 2) & 3u, sh = (pos & 3u) * 8u;
-    const u32 w0 = k == 0u ? a.x : k == 1u ? a.y : k == 2u ? a.z : a.w;
-    const u32 w1 = k == 0u ? a.y : k == 1u ? a.z : k == 2u ? a.w : b.x;
-    const u32 w2 = k == 0u ? a.z : k == 1u ? a.w : k == 2u ? b.x : b.y;
-#if defined(__CUDA_ARCH__)
-    const u32 lo = __funnelshift_r(w0, w1, sh), hi = __funnelshift_r(w1, w2, sh);
-#else
-    const u32 lo = sh ? (w0 >> sh) | (w1 << (32u - sh)) : w0, hi = sh ? (w1 >> sh) | (w2 << (32u - sh)) : w1;
-#endif
-    return (u64)lo | ((u64)hi << 32);
-  }
-};
-
 // R1, one lane: scan the top-level fields of message entry `me` and append its children.
 template <class SH>
 GGR_DEV void coop_scan_message(SH& S, const DecCtx& cx, u32 me) {
@@ -217,19 +175,11 @@ GGR_DEV void coop_scan_message(SH& S, const DecCtx& cx, u32 me) {
   u32 prev = 0xFFFFu;  // previous child entry
   bool any = false;
   const u32 end_al = (lim + 15u) & ~15u;  // the item's bytes are readable up to the end of their last 16-byte chunk
-#if COOP_WIN_CACHE
-  CoopWinCache cw;
-  cw.base = 0xFFFFFFFFu;
-#endif
   while (pos < lim) {
     // the field header out of one 8-byte window; what does not fit it is decoded byte by byte
     u32 wtag = 0, wtl = 0, wbody = 0, wvend = 0;
     bool wzero = false;
-#if COOP_WIN_CACHE
-    const u64 win = cw.get(in, pos, end_al);
-#else
     const u64 win = coop_window(in, pos, end_al);
-#endif
     const bool fast = coop_header(win, pos, &wtag, &wtl, &wbody, &wvend, &wzero) && wvend <= lim && wbody <= lim;
     u64 tag = wtag;
     if (fast) pos += wtl;
@@ -450,14 +400,6 @@ GGR_DEV int coop_leaf_value(W& w, const DecCtx& cx, const CoopEnt& e, const Fiel
   return scalar_value<W, true>(w, cx, r, e.vend, f.kind, f.child, false, &z);
 }
 
-// text size of a leaf value whose formatter is large (floats, timestamps); -1: the value is refused
-GGR_DEVN i32 coop_leaf_size_cold(const DecCtx& cx, const CoopEnt& e, const FieldD& f) {
-  Cnt c;
-  c.pos = 0;
-  if (coop_leaf_value(c, cx, e, f) != GST_OK) return -1;
-  return (i32)c.pos;
-}
-
 // ---- strings that hold quotes, backslashes, control or non-ASCII bytes: one byte per lane ----
 // JSON text length of one string byte (protojson): 1, 2 (\" \\ \b \f \n \r \t) or 6 (\u00XX)
 GGR_DEV u32 coop_esc_len(u32 c) {
@@ -595,15 +537,6 @@ GGR_DEV void coop_size_leaf(SH& S, const DecCtx& cx, u32 ei, bool have_masks) {
       return;
     }
     n += c.pos;
-  } else if (COOP_COLD_LEAF && (cls == DC_FLOAT || cls == DC_TS)) {
-    // shortest-digits floats and timestamps: out of line, so that the size kernel's hot loop stays small (the kernel
-    // waits for instructions when its hot loop outgrows the instruction cache)
-    const i32 v = coop_leaf_size_cold(cx, e, f);
-    if (v < 0) {
-      COOP_BAIL(S);
-      return;
-    }
-    n += (u32)v;
   } else {
     Cnt c;
     c.pos = 0;
@@ -654,11 +587,9 @@ GGR_DEV void coop_offsets_message(SH& S, const DecCtx& cx, u32 me) {
 // groups would spend its time on the unaligned edges of every entry; plain byte stores into
 // shared memory have no edges.
 #define GGR_COOP_STAGE 8192u /* items with more text than this: per-thread kernels */
-#ifndef GGR_COOP_STAGE_BUF
 /* the writer's staging buffer; larger texts are written in place.  6144 (configs[2]: texts up to 6.0 KB) with the kernel
    compiled for 7 blocks per SM (72 registers); 8 blocks (64 registers) spilled when tuned before the H100 port */
 #define GGR_COOP_STAGE_BUF 6144u
-#endif
 struct
 #if defined(__CUDACC__)
     __align__(16)
@@ -670,7 +601,8 @@ struct
   u32 lsrc[GGR_COOP_LONG_MAX], ldst[GGR_COOP_LONG_MAX], llen[GGR_COOP_LONG_MAX];
   u32 n_long, bad;
 };
-// R4, one lane: text of entry e into the staging buffer at pad + e.off
+// R4, one lane: text of entry e into the staging buffer at pad + e.off.  Its byte copies switch to words from 24 bytes
+// on (faster than 12 when tuned before the H100 port).
 GGR_DEV int coop_write_entry(CoopStage& E, const DecCtx& cx, const CoopEnt& e, u8* B) {
   Sw w;
   w.init(B, e.off);
@@ -685,7 +617,7 @@ GGR_DEV int coop_write_entry(CoopStage& E, const DecCtx& cx, const CoopEnt& e, u
     if (cx.flags & GGR_F_COMMA_SPACE) w.put1(' ');
   }
   if (!(e.flags & CF_ARR_ELEM) || (e.flags & CF_ARR_FIRST)) {
-    coop_copy_bytes(B + w.pos, cx.T.pool + f.name_off, f.name_len);
+    coop_copy_bytes<24u>(B + w.pos, cx.T.pool + f.name_off, f.name_len);
     w.pos += f.name_len;
   }
   if (e.flags & CF_ARR_FIRST) w.put1('[');
@@ -715,7 +647,7 @@ GGR_DEV int coop_write_entry(CoopStage& E, const DecCtx& cx, const CoopEnt& e, u
       }
     }
     if (!handed) {
-      coop_copy_bytes(B + w.pos, cx.in + e.body, len);
+      coop_copy_bytes<24u>(B + w.pos, cx.in + e.body, len);
     }
     w.pos += len;
     w.put1('"');
@@ -892,25 +824,8 @@ GGR_DEV int coop_write_item(CoopStage& E, const DecCtx& cx, const U4* tab, u32 n
     E.bad = 0;
   }
   WP_SYNC();
-#ifndef COOP_WRITE_PIPE
-#define COOP_WRITE_PIPE 0 /* 1: the next round's saved entry is requested one round ahead (slower when tuned before the H100 port, not used) */
-#endif
-  U4 an, bn;
-  an.x = an.y = an.z = an.w = bn.x = bn.y = bn.z = bn.w = 0u;
-  if (COOP_WRITE_PIPE && lane < n) {
-    an = tab[2 * lane];
-    bn = tab[2 * lane + 1];
-  }
   for (u32 i = lane; i < n; i += 32) {
-#if COOP_WRITE_PIPE
-    const U4 a = an, b = bn;
-    if (i + 32u < n) {
-      an = tab[2 * (i + 32u)];
-      bn = tab[2 * (i + 32u) + 1];
-    }
-#else
     const U4 a = tab[2 * i], b = tab[2 * i + 1];
-#endif
     CoopEnt e;
     e.vpos = a.x; e.vend = a.y; e.body = a.z; e.size = a.w;
     e.off = b.x; e.parent = (u16)b.y; e.next = (u16)(b.y >> 16);

@@ -21,9 +21,6 @@
 // owns the error semantics).
 #pragma once
 #include "ggr_encode.cuh"
-#ifndef COOP_WORD_COPY_MIN
-#define COOP_WORD_COPY_MIN 8u /* request emitter: faster than 12 when tuned before the H100 port */
-#endif
 #include "ggr_warp.cuh"
 
 #define CE_MAX_DEPTH 24
@@ -1208,18 +1205,12 @@ GGR_DEV bool ce_parse_item(SH& S, const CeLut& lut, const Tables& T, u32 root_ms
 // write nodes independently (one lane per node); long plain strings are then copied by the whole
 // warp, 128 bytes per step.
 // ------------------------------------------------------------------------------------------------
-#ifndef CE_LONG_STR
 #define CE_LONG_STR 128u /* plain strings of at least this many bytes are copied by the whole warp (faster than 96 when tuned before the H100 port) */
-#endif
-#ifndef CE_LONG_MAX
 #define CE_LONG_MAX 32u
-#endif
 #define CE_STAGE 8192u /* items with more wire bytes than this: per-thread emitter */
-#ifndef CE_STAGE_BUF
 /* the emitter's staging buffer; larger items (up to CE_STAGE and beyond) are written in place.  4864 + the lists = 5.3 KB per
    warp = 10 blocks per SM instead of 6 with 8192 (configs[2]: wire items up to 4.6 KB) */
 #define CE_STAGE_BUF 4864u
-#endif
 struct
 #if defined(__CUDACC__)
     __align__(16)
@@ -1236,7 +1227,7 @@ struct
 // STAGED: byte position p of the item lands in the staging buffer (plain shared-memory stores); otherwise - items too
 // large to stage - at G[p], the destination itself shifted so that the same positions apply (two instances: a pointer
 // that may be either makes every store a generic one, much slower on configs[2] when tuned before the H100 port)
-// nd, off: node i and its offset, loaded by the caller (one round ahead: CE_EMIT_PIPE)
+// nd, off: node i and its offset, loaded by the caller (one round ahead: CE_EMIT_LOOP)
 template <bool STAGED>
 GGR_DEV void ce_emit_node(CoopEmit& E, u8* G, const u8* in, u32 end, const u8* ir, const u32* ioff, u32 i, u32 pad, const U4 nd, const u32 off) {
   u8* const B = STAGED ? E.buf : G;
@@ -1290,8 +1281,8 @@ GGR_DEV void ce_emit_node(CoopEmit& E, u8* G, const u8* in, u32 end, const u8* i
             handed = true;
           }
         }
-        if (!handed) {
-          coop_copy_bytes(B + w.pos, in + nd.x + 1u, nd.y);
+        if (!handed) {  // words from 8 bytes on: faster than 12 when tuned before the H100 port
+          coop_copy_bytes<8u>(B + w.pos, in + nd.x + 1u, nd.y);
         }
       }
       break;
@@ -1360,11 +1351,7 @@ GGR_DEV void ce_unescape_coop(const u8* in, u32 src, u8* d, u32 dec_len) {
 
 // One item, all 32 lanes: size bytes to dst.  Items that fit the staging buffer are assembled there and leave with one
 // bulk copy; larger ones (second tier of the walker: tens of KB of wire) are written in place.
-#ifndef CE_EMIT_PIPE
-#define CE_EMIT_PIPE 1 /* the next round's node and offset are requested while this round's node is written (0: A/B builds) */
-#endif
-// one lane per node, nodes 1 .. n_nodes - 1
-#if CE_EMIT_PIPE
+// one lane per node, nodes 1 .. n_nodes - 1: the next round's node and offset are requested while this round's node is written
 #define CE_EMIT_LOOP(STG, GP)                                                             \
   do {                                                                                    \
     U4 ndn;                                                                               \
@@ -1384,10 +1371,6 @@ GGR_DEV void ce_unescape_coop(const u8* in, u32 src, u8* d, u32 dec_len) {
       ce_emit_node<STG>(E, GP, in, end, ir, ioff, i, pad, nd_, off_);                     \
     }                                                                                     \
   } while (0)
-#else
-#define CE_EMIT_LOOP(STG, GP) \
-  for (u32 i = 1 + lane; i < n_nodes; i += 32) ce_emit_node<STG>(E, GP, in, end, ir, ioff, i, pad, node_load(ir, i), ioff[i])
-#endif
 
 GGR_DEV void ce_emit_item(CoopEmit& E, const u8* in, u32 end, const u8* ir, const u32* ioff, u32 n_nodes, u8* dst, u32 size) {
   const u32 lane = wp_lane();

@@ -79,9 +79,7 @@ k_decode_coop_size(const u8* __restrict__ blob, long long n, u32 n_msgs, const i
 }
 
 #define COOP_WRITE_WARPS 4
-#ifndef COOP_WRITE_MINB
 #define COOP_WRITE_MINB 7
-#endif
 __global__ void __launch_bounds__(COOP_WRITE_WARPS * 32, COOP_WRITE_MINB)
 k_decode_coop_write(const u8* __restrict__ blob, long long n, const u8* __restrict__ in, const u64* __restrict__ in_off,
                     u32 flags, const u32* __restrict__ size, const u32* __restrict__ mode, i32* __restrict__ status,

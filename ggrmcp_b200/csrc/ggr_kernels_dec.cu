@@ -4,9 +4,7 @@
 #include "ggr_scan.cuh"
 
 // resident blocks per SM the per-thread reply kernels are compiled for (register cap = 65536 / (128 * GGR_DEC_MINB))
-#ifndef GGR_DEC_MINB
 #define GGR_DEC_MINB 8
-#endif
 
 __global__ void __launch_bounds__(GGR_BLOCK, GGR_DEC_MINB)
 k_decode_size(const u8* __restrict__ blob, long long n, u32 n_msgs, const i32* __restrict__ msg_id,

@@ -3,9 +3,7 @@
 #include "ggr_encode.cuh"
 #include "ggr_scan.cuh"
 
-#ifndef GGR_PARSE_MINB
 #define GGR_PARSE_MINB 4
-#endif
 __global__ void __launch_bounds__(GGR_BLOCK, GGR_PARSE_MINB)
 k_encode_parse(const u8* __restrict__ blob, long long n, u32 n_msgs, const i32* __restrict__ msg_id,
                const u8* __restrict__ in, const u64* __restrict__ in_off, u8* __restrict__ ir,

@@ -8,15 +8,9 @@
 #include "ggr_walk.cuh"
 
 #define CW_WARPS 4
-#ifndef CW_TOK_BLOCKS
 #define CW_TOK_BLOCKS 8
-#endif
-#ifndef CW_PLACE_BLOCKS
 #define CW_PLACE_BLOCKS 12
-#endif
-#ifndef CW_WALK_BLOCKS
 #define CW_WALK_BLOCKS 6 /* 80 registers, no spills; 7 or 8 blocks per SM spilled when tuned before the H100 port */
-#endif
 
 __global__ void __launch_bounds__(CW_WARPS * 32, CW_TOK_BLOCKS)
 k_encode_tok3(const u8* __restrict__ in, const u64* __restrict__ in_off, u8* __restrict__ ir, const u32* __restrict__ list,

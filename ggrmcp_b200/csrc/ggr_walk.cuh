@@ -117,10 +117,8 @@ GGR_DEV u32 cw_next(u32 T, u32 A) { return ((~T & 0x3FFFFu) + (A << 1)) & T; }
 // ---- the item's text travels global -> shared memory by bulk asynchronous copies (cp.async.bulk, the TMA's 1-D form)
 // that complete on an mbarrier: two tiles of CW_TILE bytes per warp, tile t + 2 is requested as soon as every lane has
 // taken its 16 bytes of the last round of tile t, so that the copy of the next tiles runs under the mask arithmetic of
-// the current one and the lanes read their chunks with one conflict-free LDS.128 instead of a global load each.
-#ifndef CW_TOK_TMA
-#define CW_TOK_TMA 1                  /* 0: every lane loads its 16 bytes from global memory itself (the round-1/2 form) */
-#endif
+// the current one and the lanes read their chunks with one conflict-free LDS.128 instead of a global load each.  The host
+// simulation has no bulk copies: there every lane loads its 16 bytes from the text itself.
 #define CW_TILE 2048u                 /* 128 chunks of 16 bytes = 4 rounds of the warp */
 #define CW_TILE_CHUNKS (CW_TILE / 16u)
 struct
@@ -190,7 +188,7 @@ GGR_DEV void cw_tok_item(CwTile* tl, u32& ph, const CwLut& LT, const u8* in, u32
   u32 k_carry = 0;                                            // kind of the last token so far (0: none yet; 7 colon, 8 comma)
   u32 tbase = 0, qbase = 0, dbase = 0, ebase = 0;
   u32 bail = 0;
-#if defined(__CUDA_ARCH__) && CW_TOK_TMA
+#if defined(__CUDA_ARCH__)
   const u32 ntiles = (nchunks + CW_TILE_CHUNKS - 1u) / CW_TILE_CHUNKS;
   if (lane == 0) {  // the first two tiles are on their way before the first round starts
     cw_tile_issue(tl, 0, in, (nchunks < CW_TILE_CHUNKS ? nchunks : CW_TILE_CHUNKS) << 4);
@@ -207,7 +205,7 @@ GGR_DEV void cw_tok_item(CwTile* tl, u32& ph, const CwLut& LT, const u8* in, u32
     const u32 ci = cb + lane;
     const u32 off = ci << 4;
     u32 Q = 0, B = 0, X = 0, W = 0xFFFFu, D = 0, HI = 0, XO = 0, XC = 0, XY = 0, XN = 0;
-#if defined(__CUDA_ARCH__) && CW_TOK_TMA
+#if defined(__CUDA_ARCH__)
     U4 v;
     v.x = v.y = v.z = v.w = 0;
     {
@@ -536,9 +534,6 @@ enum {
   CW_LEAF = 5, CW_ELEAF = 6, CW_SKIP = 7                            // ELEAF: map entry with a scalar value; SKIP: null
 };
 
-#ifndef CW_TYPE_PRE
-#define CW_TYPE_PRE 0 /* 1: token, key and string quote entries of every record fetched with full lanes before the level pass (slower when tuned before the H100 port, not used) */
-#endif
 template <int MN>
 struct CoopWalkT {
   static const u32 MAX_NODE = MN;
@@ -552,12 +547,6 @@ struct CoopWalkT {
   u8 hdr[MN];      // containers: bytes in front of the children's payload (leaves: tag length until closed)
   u32 body[MN];    // W3: containers: oneof mask, leaves: full size; W4: containers: payload; W5: absolute offset
   u32 ssz[MN];     // W3: containers: mask of fields seen; W4: sizes by slot, then offsets within the parent
-  // W3 prologue (first two tiers): the value's token and its member key, fetched for ALL records with full lanes before
-  // the level-by-level pass, whose lanes then start at the key's text instead of three dependent loads further up
-  static const bool PRE = CW_TYPE_PRE && MN <= 1024;
-  u32 tokw[PRE ? MN : 1];   // token of the value
-  u32 kinfo[PRE ? MN : 1];  // cw_key_pack of the member's key (0: no key or not a plain one)
-  u32 vinfo[PRE ? MN : 1];  // string values: cw_str_pack of the value
   u32 lvl_beg[CW_LEVELS + 2], lvl_cur[CW_LEVELS + 2];
   u32 bail, n_extra, cap;
 };
@@ -924,13 +913,12 @@ GGR_DEV u32 cw_str_pack(const CwIndex& X, u32 t) {
   const u32 nesc = (q1.esc - q0.esc) & 0xFFFFu, raw = (q1.pos - K3_POS(t) - 1u) & 0xFFFFu;
   return (q0.slow == q1.slow && nesc < 0x8000u) ? (raw | (nesc << 16) | 0x80000000u) : 0u;
 }
-// vinf: cw_str_pack(X, t) when have_vinf (fetched by the prologue of W3), else computed here
 template <bool FULL>
-GGR_DEV bool cw_leaf(const Tables& T, const CwIndex& X, const u8* in, u32 end, const FieldD& f, u32 t, CwLeaf* l, u32 vinf = 0, bool have_vinf = false) {
+GGR_DEV bool cw_leaf(const Tables& T, const CwIndex& X, const u8* in, u32 end, const FieldD& f, u32 t, CwLeaf* l) {
   const u32 k = K3_KIND(t), pos = K3_POS(t);
   if (f.kind == GK_STRING) {
     if (k != K3_STR) return false;
-    if (!have_vinf) vinf = cw_str_pack(X, t);
+    const u32 vinf = cw_str_pack(X, t);
     if (!(vinf >> 31)) return FULL ? cw_leaf_rare(T, X, in, end, f, t, l) : false;  // \u escapes, control characters
     const u32 nesc = (vinf >> 16) & 0x7FFFu;
     const u32 len = (vinf & 0xFFFFu) - nesc;  // a simple escape decodes 2 bytes to 1
@@ -1099,13 +1087,6 @@ GGR_DEV bool cw_type_item(SH& S, const Tables& T, u32 root_msg, const u8* in, u3
     S.par[pos] = pd == CW_NONE ? (u16)CW_NONE : S.slot[pd];
     // the first child of a container is the next record of the document
     if (r + 1u < n_rec && (u32)S.aux[r + 1u] == r) S.first[pos] = S.slot[r + 1u];
-    if (SH::PRE) {  // full lanes, every record's chain of loads in flight at once
-      const u32 i = S.gfield[r];
-      const u32 t = cw_ldg(X.tok + i);
-      S.tokw[pos] = t;
-      S.kinfo[pos] = (K3_V(t) && i != 0u) ? cw_key_pack(X, i) : 0u;
-      S.vinfo[pos] = K3_KIND(t) == K3_STR ? cw_str_pack(X, t) : 0u;
-    }
   }
   WP_SYNC();
   // ---- W3: types, top-down ----
@@ -1130,7 +1111,7 @@ GGR_DEV bool cw_type_item(SH& S, const Tables& T, u32 root_msg, const u8* in, u3
         const u32 i = S.vtok[r];
         p = S.par[r];
         pc = S.cls[p];
-        const u32 t = SH::PRE ? S.tokw[r] : cw_ldg(X.tok + i);
+        const u32 t = cw_ldg(X.tok + i);
         const u32 k = K3_KIND(t);
         bool ok = true;
         u32 gf = 0, cls = CW_SKIP, aux = 0, hdr = 0, body = 0;
@@ -1141,7 +1122,7 @@ GGR_DEV bool cw_type_item(SH& S, const Tables& T, u32 root_msg, const u8* in, u3
         bool is_ts = false;
         if (pc == CW_MSG || pc == CW_EMSG) {
           // member of a message: "key" : value
-          const u32 kinf = SH::PRE ? S.kinfo[r] : cw_key_pack(X, i);
+          const u32 kinf = cw_key_pack(X, i);
           if (!(kinf >> 31)) ok = (CW_WHY(101), false);  // escapes in a key: the other tiers
           const MsgD md = ggr_msg(T, S.aux[p]);
           i32 ei = 0;
@@ -1247,7 +1228,7 @@ GGR_DEV bool cw_type_item(SH& S, const Tables& T, u32 root_msg, const u8* in, u3
           if (!FULL || !cw_ts_leaf(X, in, end, t, f.tag, f.tag_len, ir, io, r, n_rec, &S.n_extra, S.cap, &body)) ok = (CW_WHY(119), false);
         } else if (ok && (cls == CW_LEAF || cls == CW_ELEAF)) {
           CwLeaf l;
-          if ((k != K3_STR && k != K3_SCALAR) || !cw_leaf<FULL>(T, X, in, end, f, t, &l, SH::PRE ? S.vinfo[r] : 0u, SH::PRE)) {
+          if ((k != K3_STR && k != K3_SCALAR) || !cw_leaf<FULL>(T, X, in, end, f, t, &l)) {
             ok = (CW_WHY(117), false);
           } else if (cls == CW_LEAF) {
             const bool packed = pc == CW_LISTP;

@@ -274,12 +274,12 @@ GGR_DEV void coop_copy_words(const u8* in, u32 src, u8* d, u32 len) {
 // One lane: len bytes of read-only data at s to d, four at a time - head bytes until d is word aligned, then aligned
 // word loads of the source brought into place by a funnel shift and one word store each (a byte loop was a large share of
 // the reply write kernel's and the request emitter's instructions).  A source word is only loaded
-// when it holds at least one byte of [s, s + len).
-#ifndef COOP_WORD_COPY_MIN
-#define COOP_WORD_COPY_MIN 12u /* shorter runs: byte by byte */
-#endif
+// when it holds at least one byte of [s, s + len).  Runs shorter than WORD_MIN are copied byte by byte.  The kernels pass
+// the threshold that measured fastest for them (24 in the reply writer, 8 in the request emitter); 12 is the general one
+// they were tuned from, for callers without a tuned value.
+template <u32 WORD_MIN = 12u>
 GGR_DEV void coop_copy_bytes(u8* d, const u8* s, u32 len) {
-  if (len >= COOP_WORD_COPY_MIN) {
+  if (len >= WORD_MIN) {
     const u32 head = (4u - (u32)((uintptr_t)d & 3u)) & 3u;
     for (u32 j = 0; j < head; j++) d[j] = s[j];
     d += head;

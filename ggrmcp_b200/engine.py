@@ -12,7 +12,7 @@ import os
 import numpy as np
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-_LIB_PATH = os.environ.get("GGR_LIB_PATH") or os.path.join(HERE, "libggrmcp_b200.so")  # override: A/B builds only (scripts/build_variant.sh)
+_LIB_PATH = os.environ.get("GGR_LIB_PATH") or os.path.join(HERE, "libggrmcp_b200.so")  # override: another build for A/B runs (scripts/ab_variants.sh)
 
 F_COMMA_SPACE = 1
 F_GRPC_FRAME = 2  # 5-byte gRPC message header in front of every request wire / reply wire item

@@ -601,13 +601,17 @@ extern "C" int hs_copy_selftest(uint32_t max_len) {
         uint8_t* dbase = (uint8_t*)(((uintptr_t)dst_raw.data() + 15) & ~(uintptr_t)15);
         uint8_t* s = sbase + 16 + sa;
         for (uint32_t i = 0; i < len; i++) s[i] = (uint8_t)(1 + (i * 7 + sa * 3 + da) % 251);
-        memset(dbase, 0xAB, 2048);
         uint8_t* d = dbase + 32 + da;
-        coop_copy_bytes(d, s, len);
-        for (uint32_t i = 0; i < 2048; i++) {
-          const bool inside = dbase + i >= d && dbase + i < d + len;
-          const uint8_t w = inside ? s[dbase + i - d] : 0xAB;
-          if (dbase[i] != w) return 1000000 + (int)(sa * 100000 + da * 10000 + len);
+        for (int k = 0; k < 3; k++) {  // word-copy thresholds: the general one, the request emitter's, the reply writer's
+          memset(dbase, 0xAB, 2048);
+          if (k == 0) coop_copy_bytes(d, s, len);
+          else if (k == 1) coop_copy_bytes<8u>(d, s, len);
+          else coop_copy_bytes<24u>(d, s, len);
+          for (uint32_t i = 0; i < 2048; i++) {
+            const bool inside = dbase + i >= d && dbase + i < d + len;
+            const uint8_t w = inside ? s[dbase + i - d] : 0xAB;
+            if (dbase[i] != w) return 1000000 + (int)(sa * 100000 + da * 10000 + len);
+          }
         }
         // the whole-warp form of the same copy
         memset(dbase, 0xAB, 2048);

@@ -562,8 +562,9 @@ def test_decode_unsorted_maps(oracle, hsim):
 
 
 def test_byte_run_copies(hsim):
-    """coop_copy_bytes / coop_copy_words (ggr_warp.cuh): every source and destination alignment, every length up to 300,
-    against a byte-wise reference; nothing outside the destination run may change"""
+    """coop_copy_bytes (with the general word-copy threshold and the two the kernels use) / coop_copy_words (ggr_warp.cuh):
+    every source and destination alignment, every length up to 300, against a byte-wise reference; nothing outside the
+    destination run may change"""
     import ctypes as C
     import hostsim
     L = hostsim.lib()
