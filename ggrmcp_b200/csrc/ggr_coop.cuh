@@ -586,8 +586,7 @@ GGR_DEV void coop_offsets_message(SH& S, const DecCtx& cx, u32 me) {
 // stores.  Entries are small (a key and a few dozen bytes), so a streaming writer with aligned
 // groups would spend its time on the unaligned edges of every entry; plain byte stores into
 // shared memory have no edges.
-#define GGR_COOP_STAGE 8192u /* items with more text than this: per-thread kernels */
-/* the writer's staging buffer; larger texts are written in place.  6144 (configs[2]: texts up to 6.0 KB) with the kernel
+/* the writer's staging buffer; larger texts, of any size, are written in place.  6144 (configs[2]: texts up to 6.0 KB) with the kernel
    compiled for 7 blocks per SM (72 registers); 8 blocks (64 registers) spilled when tuned before the H100 port */
 #define GGR_COOP_STAGE_BUF 6144u
 struct
