@@ -171,11 +171,14 @@ struct DevBuf {
 };
 
 struct Scratch {
-  DevBuf ir, size, aux, sums, pend, ioff, nn;
-  DevBuf wtext, woff, wsize;  // result wrapping: protojson texts, their offsets, body sizes
-  DevBuf sortpool;            // reply side: (key, position) records of maps whose entries arrive unsorted
-  DevBuf tabpool, taboff;     // reply side, second lock-step tier: pooled entry tables and where each item's table starts
-  DevBuf spread;              // per-thread kernels: the list of large items, one per warp (k_spread)
+  DevBuf all[14];
+  DevBuf &ir = all[0], &size = all[1], &aux = all[2], &sums = all[3], &pend = all[4], &ioff = all[5], &nn = all[6];
+  DevBuf &wtext = all[7], &woff = all[8], &wsize = all[9];  // result wrapping: protojson texts, their offsets, body sizes
+  DevBuf& sortpool = all[10];  // reply side: (key, position) records of maps whose entries arrive unsorted
+  DevBuf &tabpool = all[11], &taboff = all[12];  // reply side, second lock-step tier: pooled entry tables and where each item's table starts
+  DevBuf& spread = all[13];                      // per-thread kernels: the list of large items, one per warp (k_spread)
+  Scratch() = default;
+  Scratch(const Scratch&) = delete;
 };
 #define GGR_MAX_SLOTS 8
 #define GGR_SPREAD_CAP 16384u /* large items that get a warp each per call and direction; the rest stay 32 to a warp */
@@ -240,16 +243,35 @@ struct ggr_engine {
   std::vector<Span> spans;
 };
 
-static cudaEvent_t prof_mark(ggr_engine* e, cudaStream_t st, size_t* idx) {
-  if (e->ev_used == e->ev_pool.size()) {
-    cudaEvent_t ev;
-    cudaEventCreate(&ev);
-    e->ev_pool.push_back(ev);
+// Profile slots, as include/ggrmcp_b200.h and engine.py's KERNELS name them
+enum ProfSlot {
+  P_ENCODE_PARSE, P_ENCODE_SCAN, P_ENCODE_EMIT, P_DECODE_SIZE, P_DECODE_SCAN, P_DECODE_WRITE, P_DECODE_COOP_SIZE, P_DECODE_COOP_WRITE,
+  P_ENCODE_COOP_PARSE, P_ENCODE_BLOCK_SUMS, P_ENCODE_COOP_EMIT, P_ENCODE_COOP_TOK, P_ENCODE_PLACE, P_ENCODE_TYPE
+};
+// Per-kernel timing of one call: span(slot) times what the stream ran since the previous mark() or span()
+struct Prof {
+  ggr_engine* e;
+  cudaStream_t st;
+  bool on;
+  size_t last = 0;
+  Prof(ggr_engine* e_, cudaStream_t st_) : e(e_), st(st_), on(e_->profiling && e_->ev_used + 16 <= 65536) {}
+  void mark() {
+    if (!on) return;
+    if (e->ev_used == e->ev_pool.size()) {
+      cudaEvent_t ev;
+      cudaEventCreate(&ev);
+      e->ev_pool.push_back(ev);
+    }
+    last = e->ev_used++;
+    cudaEventRecord(e->ev_pool[last], st);
   }
-  *idx = e->ev_used++;
-  cudaEventRecord(e->ev_pool[*idx], st);
-  return e->ev_pool[*idx];
-}
+  void span(ProfSlot slot) {
+    if (!on) return;
+    const size_t a = last;
+    mark();
+    e->spans.push_back({slot, a, last});
+  }
+};
 
 // the caller's current device is put back when an entry point returns
 struct DeviceGuard {
@@ -281,6 +303,62 @@ static bool ensure(ggr_engine* e, DevBuf& b, size_t bytes) {
   if (!cuda_ok(e, cudaMalloc(&b.p, want), "cudaMalloc")) return false;
   b.cap = want;
   return true;
+}
+
+// The lock-step work lists of a call, in sc.pend: every list's header first (zeroed together), then n item indices per list.
+struct WorkList {
+  GgrList* h;
+  u32* item;
+};
+// request side: the router's lock-step items; what the walker leaves, after all its tiers (GGR_WALK=0: after the first
+// parser tier), after its first tier and after its second; the per-thread parser's items
+struct EncodeLists {
+  WorkList lockstep, walk_left, walk1_left, walk2_left, per_thread;
+};
+// reply side: the router's lock-step items; what the first lock-step tier leaves
+struct DecodeLists {
+  WorkList lockstep, tier1_left;
+};
+// request bodies: the router's lock-step items; what the first parser tier leaves; what neither tier can take
+struct BodyLists {
+  WorkList lockstep, tier1_left, rest;
+};
+template <class Set>
+static constexpr int list_count() {
+  return sizeof(Set) / sizeof(WorkList);
+}
+template <class Set>
+static Set carve_lists(void* p, int64_t n) {
+  Set set;
+  WorkList* w = reinterpret_cast<WorkList*>(&set);
+  GgrList* h = (GgrList*)p;
+  u32* item = (u32*)(h + list_count<Set>());
+  for (int k = 0; k < list_count<Set>(); k++) w[k] = {h + k, item + (size_t)k * n};
+  return set;
+}
+template <class Set>
+static bool make_lists(ggr_engine* e, DevBuf& pend, int64_t n, cudaStream_t st, Set* set) {
+  const size_t heads = list_count<Set>() * sizeof(GgrList);
+  if (!ensure(e, pend, heads + list_count<Set>() * (size_t)n * 4) || !cuda_ok(e, cudaMemsetAsync(pend.p, 0, heads, st), "memset"))
+    return false;
+  *set = carve_lists<Set>(pend.p, n);
+  return true;
+}
+
+// What every device-buffer batch shares: the argument checks, the empty batch and the per-item scratch of every direction.
+// Then `kernels(nb)` launches the direction's kernels (nb: blocks of GGR_BLOCK items) on the engine's device.
+template <class Kernels>
+static int run_batch(ggr_engine* e, const ggr_schema* s, Scratch& sc, int64_t n, bool have_args, const uint8_t* in, const uint8_t* out,
+                     uint64_t* out_off, cudaStream_t st, Kernels kernels) {
+  if (!e || !s || n < 0 || (n > 0 && !have_args)) return GGR_ERR_INVALID_ARGUMENT;
+  if (((uintptr_t)in & 15) || ((uintptr_t)out & 7)) return GGR_ERR_INVALID_ARGUMENT;
+  DeviceGuard dg(e->device);
+  if (n == 0) return cuda_ok(e, cudaMemsetAsync(out_off, 0, sizeof(uint64_t), st), "memset") ? GGR_SUCCESS : GGR_ERR_CUDA;
+  const long long nb = (n + GGR_BLOCK - 1) / GGR_BLOCK;
+  if (!ensure(e, sc.size, (size_t)n * 4) || !ensure(e, sc.aux, (size_t)n * 4) || !ensure(e, sc.sums, (size_t)nb * 8)) return GGR_ERR_CUDA;
+  const int rc = kernels(nb);
+  if (rc != GGR_SUCCESS) return rc;
+  return cuda_ok(e, cudaGetLastError(), "kernel launch") ? GGR_SUCCESS : GGR_ERR_CUDA;
 }
 
 // ---- NUMA placement of the host side (no libnuma in the image: sysfs + sched_setaffinity + first touch) ----
@@ -353,21 +431,25 @@ static int usable_cpus() {
   if (quota > 0 && quota < n) n = (int)(quota + 0.999);
   return n < 1 ? 1 : n;
 }
+// want = the CPUs of the GPU's node that the calling thread may use now (old); false when none are known
+static bool node_mask(const ggr_engine* e, cpu_set_t* old, cpu_set_t* want) {
+  if (e->node_cpus.empty() || sched_getaffinity(0, sizeof *old, old) != 0) return false;
+  CPU_ZERO(want);
+  int n = 0;
+  for (int c : e->node_cpus)
+    if (c < CPU_SETSIZE && CPU_ISSET(c, old)) {  // stay inside what the process may use (containers, taskset)
+      CPU_SET(c, want);
+      n++;
+    }
+  return n > 0;
+}
 // binds the calling thread to the GPU's node for the lifetime of the object (old mask restored)
 struct NodeBind {
   cpu_set_t old;
   bool active = false;
   explicit NodeBind(const ggr_engine* e) {
-    if (e->node_cpus.empty() || sched_getaffinity(0, sizeof old, &old) != 0) return;
     cpu_set_t want;
-    CPU_ZERO(&want);
-    int n = 0;
-    for (int c : e->node_cpus)
-      if (c < CPU_SETSIZE && CPU_ISSET(c, &old)) {  // stay inside what the process may use (containers, taskset)
-        CPU_SET(c, &want);
-        n++;
-      }
-    if (n && sched_setaffinity(0, sizeof want, &want) == 0) active = true;
+    active = node_mask(e, &old, &want) && sched_setaffinity(0, sizeof want, &want) == 0;
   }
   ~NodeBind() {
     if (active) sched_setaffinity(0, sizeof old, &old);
@@ -379,17 +461,8 @@ extern "C" {
 int ggr_device_numa_node(const ggr_engine* e) { return e ? e->numa_node : -1; }
 int ggr_bind_thread_to_device(const ggr_engine* e) {
   if (!e) return GGR_ERR_INVALID_ARGUMENT;
-  if (e->node_cpus.empty()) return GGR_SUCCESS;  // nothing known: leave the thread alone
   cpu_set_t old, want;
-  if (sched_getaffinity(0, sizeof old, &old) != 0) return GGR_SUCCESS;
-  CPU_ZERO(&want);
-  int n = 0;
-  for (int c : e->node_cpus)
-    if (c < CPU_SETSIZE && CPU_ISSET(c, &old)) {
-      CPU_SET(c, &want);
-      n++;
-    }
-  if (n) sched_setaffinity(0, sizeof want, &want);
+  if (node_mask(e, &old, &want)) sched_setaffinity(0, sizeof want, &want);  // nothing known: the thread is left alone
   return GGR_SUCCESS;
 }
 int ggr_host_alloc(ggr_engine* e, size_t bytes, void** out) {
@@ -497,9 +570,8 @@ void ggr_engine_destroy(ggr_engine* e) {
   cudaSetDevice(e->device);
   cudaStreamSynchronize(e->stream);
   auto free_scratch = [](Scratch& sc) {
-    DevBuf* bufs[] = {&sc.ir, &sc.size, &sc.aux, &sc.sums, &sc.pend, &sc.ioff, &sc.nn, &sc.wtext, &sc.woff, &sc.wsize, &sc.sortpool, &sc.spread, &sc.tabpool, &sc.taboff};
-    for (DevBuf* b : bufs)
-      if (b->p) cudaFree(b->p);
+    for (DevBuf& b : sc.all)
+      if (b.p) cudaFree(b.p);
   };
   free_scratch(e->dev_sc[0]);
   free_scratch(e->dev_sc[1]);
@@ -620,11 +692,12 @@ int ggr_debug_paths(ggr_engine* e, int64_t n, uint32_t* reply_mode, uint32_t* re
   if (reply_mode && e->dev_sc[1].aux.p && e->dev_sc[1].aux.cap >= (size_t)n * 4)
     cudaMemcpy(reply_mode, e->dev_sc[1].aux.p, (size_t)n * 4, cudaMemcpyDeviceToHost);
   if (request_counts && e->dev_sc[0].pend.p) {
-    uint32_t c[16];
-    cudaMemcpy(c, e->dev_sc[0].pend.p, sizeof c, cudaMemcpyDeviceToHost);
-    request_counts[0] = c[0];
-    request_counts[1] = c[4];
-    request_counts[2] = c[8];
+    GgrList heads[list_count<EncodeLists>()];
+    cudaMemcpy(heads, e->dev_sc[0].pend.p, sizeof heads, cudaMemcpyDeviceToHost);
+    const EncodeLists L = carve_lists<EncodeLists>(heads, 0);  // over the host copy of the headers
+    request_counts[0] = L.lockstep.h->n;
+    request_counts[1] = L.walk_left.h->n;
+    request_counts[2] = L.per_thread.h->n;
   }
   return GGR_SUCCESS;
 }
@@ -635,13 +708,189 @@ int ggr_synchronize(ggr_engine* e) {
   return cuda_ok(e, cudaStreamSynchronize(e->stream), "cudaStreamSynchronize") ? GGR_SUCCESS : GGR_ERR_CUDA;
 }
 
-static int run_dev_kernels(ggr_engine* e, const ggr_schema* s, Scratch& sc, bool encode, int64_t n, const int32_t* msg_id, const uint8_t* in,
-                           const uint64_t* in_off, uint64_t in_bytes, uint8_t* out, uint64_t out_cap, uint64_t* out_off,
-                           int32_t* status, uint32_t flags, cudaStream_t st);
+// Request side.  Without the lock-step parser (GGR_COOP_ENC=0) the per-thread parser takes every item.  With it, the router
+// sends small and oversized items to the per-thread parser and the others down the lock-step tiers: the token-parallel
+// walker (GGR_WALK=0: the first table tier of the lock-step parser), then its large-table tier over what that left, then
+// the per-thread parser over what is still left.
+static int run_encode_kernels(ggr_engine* e, const ggr_schema* s, Scratch& sc, int64_t n, long long nb, const int32_t* msg_id,
+                              const uint8_t* in, const uint64_t* in_off, uint64_t in_bytes, uint8_t* out, uint64_t out_cap,
+                              uint64_t* out_off, int32_t* status, uint32_t flags, cudaStream_t st) {
+  const bool coop = e->use_coop_enc;
+  EncodeLists L;
+  if (!ensure(e, sc.ir, ggr_ir_bytes(in_bytes, n))) return GGR_ERR_CUDA;
+  if (coop && (!ensure(e, sc.ioff, ggr_ioff_bytes(in_bytes, n)) || !ensure(e, sc.nn, (size_t)n * 4) || !make_lists(e, sc.pend, n, st, &L) ||
+               !cuda_ok(e, cudaMemsetAsync(sc.nn.p, 0, (size_t)n * 4, st), "memset")))
+    return GGR_ERR_CUDA;
+  const u32 n_msgs = (u32)s->cs.msg_names.size();
+  const u32 frame = (flags & GGR_F_GRPC_FRAME) ? 5u : 0u;  // message header in front of every item
+  u8* ir = (u8*)sc.ir.p;
+  u32 *size = (u32*)sc.size.p, *first = (u32*)sc.aux.p, *ioff = (u32*)sc.ioff.p, *nn = (u32*)sc.nn.p;
+  u64* sums = (u64*)sc.sums.p;
+  Prof prof(e, st);
+  prof.mark();
+  if (!coop) {
+    ggr_launch_encode_parse(st, (unsigned)nb, s->d_blob, n, n_msgs, msg_id, in, in_off, ir, size, first, status, sums, nullptr, nullptr);
+    e->launches += 1;
+    if (frame) {
+      ggr_launch_frame_sizes(st, n, size, status);
+      ggr_launch_block_sums(st, (unsigned)nb, n, size, sums);
+      e->launches += 2;
+    }
+    prof.span(P_ENCODE_PARSE);
+  } else {
+    // router: small (and oversized) items straight to the per-thread parser
+    k_route<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(n, in_off, e->min_json, 65000u - 16u, L.lockstep.item, &L.lockstep.h->n,
+                                                        L.per_thread.item, &L.per_thread.h->n, nullptr);
+    if (e->use_walk) {
+      // token index, value records, then types, sizes and offsets in three tiers, each over what the one before left: the
+      // second takes large items and the other leaf forms, the third (one warp per SM) thousands of values
+      ggr_launch_encode_tok2(st, n, in, in_off, ir, L.lockstep.item, L.lockstep.h, e->sm_count);
+      prof.span(P_ENCODE_COOP_TOK);
+      ggr_launch_encode_place(st, n, in_off, ir, L.lockstep.item, L.lockstep.h, e->sm_count);
+      prof.span(P_ENCODE_PLACE);
+      ggr_launch_encode_type(st, 0, n, s->d_blob, n_msgs, msg_id, in, in_off, ir, size, first, status, ioff, nn, L.lockstep.item, L.lockstep.h,
+                             L.walk1_left.item, L.walk1_left.h, e->sm_count);
+      ggr_launch_encode_type(st, 1, n, s->d_blob, n_msgs, msg_id, in, in_off, ir, size, first, status, ioff, nn, L.walk1_left.item,
+                             L.walk1_left.h, L.walk2_left.item, L.walk2_left.h, e->sm_count);
+      ggr_launch_encode_type(st, 2, n, s->d_blob, n_msgs, msg_id, in, in_off, ir, size, first, status, ioff, nn, L.walk2_left.item,
+                             L.walk2_left.h, L.walk_left.item, L.walk_left.h, e->sm_count);
+      prof.span(P_ENCODE_TYPE);
+      e->launches += 6;
+    } else {
+      ggr_launch_encode_coop_tok(st, n, in, in_off, ir, L.lockstep.item, L.lockstep.h, e->sm_count);
+      prof.span(P_ENCODE_COOP_TOK);
+      ggr_launch_encode_coop_parse(st, 0, n, s->d_blob, n_msgs, msg_id, in, in_off, ir, size, first, status, ioff, nn, L.lockstep.item,
+                                   L.lockstep.h, L.walk_left.item, L.walk_left.h, e->sm_count, nullptr, nullptr, -1);
+      e->launches += 3;
+    }
+    ggr_launch_encode_coop_parse(st, 1, n, s->d_blob, n_msgs, msg_id, in, in_off, ir, size, first, status, ioff, nn, L.walk_left.item,
+                                 L.walk_left.h, L.per_thread.item, L.per_thread.h, e->sm_count, nullptr, nullptr, -1);
+    e->launches += 1;
+    prof.span(P_ENCODE_COOP_PARSE);
+    if (e->spread_min) {
+      // the per-thread list, split: small items 32 to a warp, large ones a warp each (k_spread)
+      size_t max_big = (size_t)(in_bytes / e->spread_min) + 1;  // items of at least spread_min bytes
+      if (max_big > GGR_SPREAD_CAP) max_big = GGR_SPREAD_CAP;
+      if (!ensure(e, sc.spread, (max_big * 32 + (size_t)n) * 4 + 64)) return GGR_ERR_CUDA;
+      u32* sp_cnt = (u32*)sc.spread.p;
+      u32* sp_list = sp_cnt + 16;
+      u32* sp_small = sp_list + max_big * 32;
+      if (!cuda_ok(e, cudaMemsetAsync(sp_cnt, 0, 64, st), "memset") || !cuda_ok(e, cudaMemsetAsync(sp_list, 0xFF, max_big * 32 * 4, st), "memset"))
+        return GGR_ERR_CUDA;
+      for (int phase = 0; phase < 2; phase++)
+        k_spread<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(phase, n, in_off, e->spread_min, L.per_thread.item, &L.per_thread.h->n, nullptr,
+                                                             sp_small, sp_list, sp_cnt, (u32)max_big);
+      ggr_launch_encode_parse(st, (unsigned)((max_big * 32 + GGR_BLOCK - 1) / GGR_BLOCK), s->d_blob, n, n_msgs, msg_id, in, in_off, ir, size,
+                              first, status, sums, sp_list, sp_cnt);
+      ggr_launch_encode_parse(st, (unsigned)nb, s->d_blob, n, n_msgs, msg_id, in, in_off, ir, size, first, status, sums, sp_small, sp_cnt + 1);
+      e->launches += 4;
+    } else {
+      ggr_launch_encode_parse(st, (unsigned)nb, s->d_blob, n, n_msgs, msg_id, in, in_off, ir, size, first, status, sums, L.per_thread.item,
+                              &L.per_thread.h->n);
+      e->launches += 1;
+    }
+    prof.span(P_ENCODE_PARSE);
+    if (frame) {
+      ggr_launch_frame_sizes(st, n, size, status);
+      e->launches += 1;
+    }
+    ggr_launch_block_sums(st, (unsigned)nb, n, size, sums);
+    e->launches += 1;
+    prof.span(P_ENCODE_BLOCK_SUMS);
+  }
+  k_scan_blocks<<<1, 1024, 0, st>>>(sums, nb, out_off + n);
+  prof.span(P_ENCODE_SCAN);
+  ggr_launch_encode_emit(st, (unsigned)nb, n, in, in_off, ir, size, first, status, sums, out, out_cap, out_off, coop ? nn : nullptr, frame);
+  prof.span(P_ENCODE_EMIT);
+  e->launches += 2;
+  if (coop) {
+    ggr_launch_encode_coop_emit(st, n, in, in_off, ir, ioff, nn, size, status, out, out_off, e->sm_count, L.lockstep.item, L.lockstep.h, frame);
+    prof.span(P_ENCODE_COOP_EMIT);
+    e->launches += 1;
+  }
+  return GGR_SUCCESS;
+}
+
+// Reply side: the lock-step kernels (two tiers; GGR_COOP=0: none) take every regular item; the per-thread kernels then
+// walk only what was left pending (irregular field order, maps, malformed wire, ...).
+static int run_decode_kernels(ggr_engine* e, const ggr_schema* s, Scratch& sc, int64_t n, long long nb, const int32_t* msg_id,
+                              const uint8_t* in, const uint64_t* in_off, uint64_t in_bytes, uint8_t* out, uint64_t out_cap,
+                              uint64_t* out_off, int32_t* status, uint32_t flags, cudaStream_t st) {
+  const bool coop = e->use_coop;
+  const u32 n_msgs = (u32)s->cs.msg_names.size();
+  Prof prof(e, st);
+  prof.mark();
+  // a map entry takes at least 4 bytes of wire; both passes sort, the fast walk may give way to the slow one
+  const uint64_t want_recs = in_bytes / 4 * 3 + 1024;
+  const uint32_t sort_cap = (uint32_t)(want_recs > 0x3FFFFFFFull ? 0x3FFFFFFFull : want_recs);
+  if (!ensure(e, sc.sortpool, (size_t)sort_cap * 16 + 16)) return GGR_ERR_CUDA;
+  if (!cuda_ok(e, cudaMemsetAsync(sc.sortpool.p, 0, 16, st), "memset")) return GGR_ERR_CUDA;
+  DecodeLists L;
+  if (coop) {
+    // second tier's tables: a field occurrence takes at least 2 bytes of wire; the pool is capped at 4 M entries (128 MB)
+    const uint64_t want_ent = in_bytes / 2 + 4096;
+    const uint32_t pool_cap = (uint32_t)(want_ent > (4ull << 20) ? (4ull << 20) : want_ent);
+    if (!ensure(e, sc.ir, ggr_decode_coop_table_bytes(n)) || !ensure(e, sc.nn, (size_t)n * 4) || !make_lists(e, sc.pend, n, st, &L) ||
+        !ensure(e, sc.tabpool, (size_t)pool_cap * 32 + 32) || !ensure(e, sc.taboff, (size_t)n * 4) ||
+        !cuda_ok(e, cudaMemsetAsync(sc.tabpool.p, 0, 32, st), "memset"))
+      return GGR_ERR_CUDA;
+    k_route<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(n, in_off, e->min_wire, 0x3FFFFF00u, L.lockstep.item, &L.lockstep.h->n, nullptr,
+                                                        nullptr, (u32*)sc.aux.p);
+    ggr_launch_decode_coop_size(st, n, s->d_blob, n_msgs, msg_id, in, in_off, flags, (u32*)sc.size.p, (u32*)sc.aux.p, status, sc.ir.p,
+                                (u32*)sc.nn.p, e->sm_count, L.lockstep.item, L.lockstep.h, L.tier1_left.item, L.tier1_left.h, sc.tabpool.p,
+                                pool_cap, (u32*)sc.taboff.p);
+    e->launches += 3;
+    prof.span(P_DECODE_COOP_SIZE);
+  }
+  // large items the lock-step kernels left: a warp each (k_spread), sized before and written after the pass over the batch
+  const bool spread = coop && e->spread_min != 0;
+  size_t max_big = spread ? (size_t)(in_bytes / e->spread_min) + 1 : 0;
+  if (max_big > GGR_SPREAD_CAP) max_big = GGR_SPREAD_CAP;
+  const unsigned spread_blocks = (unsigned)((max_big * 32 + GGR_BLOCK - 1) / GGR_BLOCK);
+  u32* sp_cnt = nullptr;
+  if (spread) {
+    if (!ensure(e, sc.spread, max_big * 32 * 4 + 64)) return GGR_ERR_CUDA;
+    sp_cnt = (u32*)sc.spread.p;
+    if (!cuda_ok(e, cudaMemsetAsync(sp_cnt, 0, 64, st), "memset") || !cuda_ok(e, cudaMemsetAsync(sp_cnt + 16, 0xFF, max_big * 32 * 4, st), "memset"))
+      return GGR_ERR_CUDA;
+    for (int phase = 0; phase < 2; phase++)
+      k_spread<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(phase, n, in_off, e->spread_min, nullptr, nullptr, (const u32*)sc.aux.p, nullptr,
+                                                           sp_cnt + 16, sp_cnt, (u32)max_big);
+    ggr_launch_decode_size(st, spread_blocks, s->d_blob, n, n_msgs, msg_id, in, in_off, flags, (u32*)sc.size.p, (u32*)sc.aux.p, status,
+                           (u64*)sc.sums.p, 1, sc.sortpool.p, sort_cap, sp_cnt + 16, sp_cnt);
+    e->launches += 3;
+  }
+  ggr_launch_decode_size(st, (unsigned)nb, s->d_blob, n, n_msgs, msg_id, in, in_off, flags, (u32*)sc.size.p, (u32*)sc.aux.p, status,
+                         (u64*)sc.sums.p, coop ? 1 : 0, sc.sortpool.p, sort_cap);
+  prof.span(P_DECODE_SIZE);
+  k_scan_blocks<<<1, 1024, 0, st>>>((u64*)sc.sums.p, nb, out_off + n);
+  prof.span(P_DECODE_SCAN);
+  ggr_launch_decode_write(st, (unsigned)nb, s->d_blob, n, msg_id, in, in_off, flags, (const u32*)sc.size.p, (const u32*)sc.aux.p, status,
+                          (const u64*)sc.sums.p, out, out_cap, out_off, sc.sortpool.p, sort_cap);
+  e->launches += 3;
+  if (spread) {
+    ggr_launch_decode_write(st, spread_blocks, s->d_blob, n, msg_id, in, in_off, flags, (const u32*)sc.size.p, (const u32*)sc.aux.p, status,
+                            (const u64*)sc.sums.p, out, out_cap, out_off, sc.sortpool.p, sort_cap, sp_cnt + 16, sp_cnt);
+    e->launches += 1;
+  }
+  prof.span(P_DECODE_WRITE);
+  if (coop) {
+    ggr_launch_decode_coop_write(st, n, s->d_blob, in, in_off, flags, (const u32*)sc.size.p, (const u32*)sc.aux.p, status, sc.ir.p,
+                                 (const u32*)sc.nn.p, out, out_off, e->sm_count, L.lockstep.item, L.lockstep.h, sc.tabpool.p,
+                                 (const u32*)sc.taboff.p);
+    prof.span(P_DECODE_COOP_WRITE);
+    e->launches += 1;
+  }
+  return GGR_SUCCESS;
+}
+
 static int run_dev(ggr_engine* e, const ggr_schema* s, Scratch& sc, bool encode, int64_t n, const int32_t* msg_id, const uint8_t* in,
                    const uint64_t* in_off, uint64_t in_bytes, uint8_t* out, uint64_t out_cap, uint64_t* out_off,
                    int32_t* status, uint32_t flags, cudaStream_t st) {
-  const int rc = run_dev_kernels(e, s, sc, encode, n, msg_id, in, in_off, in_bytes, out, out_cap, out_off, status, flags, st);
+  const int rc = run_batch(e, s, sc, n, msg_id && in && in_off && out_off && status, in, out, out_off, st, [&](long long nb) {
+    return (encode ? run_encode_kernels : run_decode_kernels)(e, s, sc, n, nb, msg_id, in, in_off, in_bytes, out, out_cap, out_off, status,
+                                                              flags, st);
+  });
   if (e && e->poison) {  // after the last kernel of the call, in stream order
     DevBuf* bufs[] = {&sc.ir, &sc.size, &sc.aux, &sc.sums, &sc.pend, &sc.ioff, &sc.nn};
     for (DevBuf* b : bufs) {
@@ -650,221 +899,6 @@ static int run_dev(ggr_engine* e, const ggr_schema* s, Scratch& sc, bool encode,
     }
   }
   return rc;
-}
-static int run_dev_kernels(ggr_engine* e, const ggr_schema* s, Scratch& sc, bool encode, int64_t n, const int32_t* msg_id, const uint8_t* in,
-                           const uint64_t* in_off, uint64_t in_bytes, uint8_t* out, uint64_t out_cap, uint64_t* out_off,
-                           int32_t* status, uint32_t flags, cudaStream_t st) {
-  if (!e || !s || n < 0 || (n > 0 && (!msg_id || !in || !in_off || !out_off || !status))) return GGR_ERR_INVALID_ARGUMENT;
-  if (((uintptr_t)in & 15) || ((uintptr_t)out & 7)) return GGR_ERR_INVALID_ARGUMENT;
-  DeviceGuard dg(e->device);
-  if (n == 0) {
-    return cuda_ok(e, cudaMemsetAsync(out_off, 0, sizeof(uint64_t), st), "memset") ? GGR_SUCCESS : GGR_ERR_CUDA;
-  }
-  long long nb = (n + GGR_BLOCK - 1) / GGR_BLOCK;
-  if (!ensure(e, sc.size, (size_t)n * 4) || !ensure(e, sc.aux, (size_t)n * 4) || !ensure(e, sc.sums, (size_t)nb * 8)) return GGR_ERR_CUDA;
-  if (encode && !ensure(e, sc.ir, (size_t)in_bytes * 8 + (size_t)n * 128 + 256)) return GGR_ERR_CUDA;
-  u32 n_msgs = (u32)s->cs.msg_names.size();
-  const bool prof = e->profiling && e->ev_used + 16 <= 65536;
-  const u32 frame = (encode && (flags & GGR_F_GRPC_FRAME)) ? 5u : 0u;  // request side: message header in front of every item
-  size_t m0 = 0, m1 = 0, m2 = 0, m3 = 0, mx = 0;
-  bool have_mx = false;
-  if (prof) prof_mark(e, st, &m0);
-  if (encode) {
-    if (e->use_coop_enc) {
-      // lock-step parser first (one warp per item); what it leaves goes to the per-thread parser
-      if (!ensure(e, sc.pend, (size_t)n * 20 + 128) || !ensure(e, sc.ioff, (size_t)in_bytes * 2 + (size_t)n * 32 + 64) ||
-          !ensure(e, sc.nn, (size_t)n * 4))
-        return GGR_ERR_CUDA;
-      // [0] lock-step items, [4] left by the walker (all tiers), [8] per-thread items, [12] left by the walker's first tier,
-      // [16] left by its second tier; each list length is followed by the ticket counters of the kernels that run over the list
-      u32* counters = (u32*)sc.pend.p;
-      u32* big = counters + 32;
-      u32* pend1 = big + n;
-      u32* pend2 = pend1 + n;
-      u32* pend1b = pend2 + n;
-      u32* pend1c = pend1b + n;
-      size_t c0 = 0, c1 = 0;
-      if (!cuda_ok(e, cudaMemsetAsync(counters, 0, 128, st), "memset") ||
-          !cuda_ok(e, cudaMemsetAsync(sc.nn.p, 0, (size_t)n * 4, st), "memset"))
-        return GGR_ERR_CUDA;
-      if (prof) prof_mark(e, st, &m0);
-      // router: small (and oversized) items straight to the per-thread parser
-      k_route<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(n, in_off, e->min_json, 65000u - 16u, big, counters, pend2, counters + 8, nullptr);
-      size_t t1 = 0, t_tok = 0;
-      if (e->use_walk) {
-        // token index, then the token-parallel walker (ggr_walk.cuh); what it leaves: the fused large-table kernel
-        ggr_launch_encode_tok2(st, n, in, in_off, (u8*)sc.ir.p, big, counters, e->sm_count);
-        if (prof) prof_mark(e, st, &t1);
-        t_tok = t1;
-        ggr_launch_encode_place(st, n, in_off, (u8*)sc.ir.p, big, counters, e->sm_count);
-        size_t t2 = 0, t3 = 0;
-        if (prof) prof_mark(e, st, &t2);
-        ggr_launch_encode_type(st, 0, n, s->d_blob, n_msgs, msg_id, in, in_off, (u8*)sc.ir.p, (u32*)sc.size.p, (u32*)sc.aux.p, status,
-                               (u32*)sc.ioff.p, (u32*)sc.nn.p, big, counters, pend1b, counters + 12, e->sm_count);
-        // second tier over what the first left (large items, the other leaf forms), third tier (thousands of values, one warp
-        // per SM) over what the second left; what that leaves: pend1 -> the fused kernel
-        ggr_launch_encode_type(st, 1, n, s->d_blob, n_msgs, msg_id, in, in_off, (u8*)sc.ir.p, (u32*)sc.size.p, (u32*)sc.aux.p, status,
-                               (u32*)sc.ioff.p, (u32*)sc.nn.p, pend1b, counters + 12, pend1c, counters + 16, e->sm_count);
-        ggr_launch_encode_type(st, 2, n, s->d_blob, n_msgs, msg_id, in, in_off, (u8*)sc.ir.p, (u32*)sc.size.p, (u32*)sc.aux.p, status,
-                               (u32*)sc.ioff.p, (u32*)sc.nn.p, pend1c, counters + 16, pend1, counters + 4, e->sm_count);
-        if (prof) {
-          prof_mark(e, st, &t3);
-          e->spans.push_back({12, t1, t2});  // value records
-          e->spans.push_back({13, t2, t3});  // types, sizes, offsets
-          t1 = t3;                           // slot 8: what is left for the fused large-table kernel
-        }
-      } else {
-        ggr_launch_encode_coop_tok(st, n, in, in_off, (u8*)sc.ir.p, big, counters, e->sm_count);
-        if (prof) prof_mark(e, st, &t1);
-        t_tok = t1;
-        ggr_launch_encode_coop_parse(st, 0, n, s->d_blob, n_msgs, msg_id, in, in_off, (u8*)sc.ir.p, (u32*)sc.size.p,
-                                     (u32*)sc.aux.p, status, (u32*)sc.ioff.p, (u32*)sc.nn.p, big, counters, pend1, counters + 4, e->sm_count, nullptr, nullptr, -1);
-      }
-      ggr_launch_encode_coop_parse(st, 1, n, s->d_blob, n_msgs, msg_id, in, in_off, (u8*)sc.ir.p, (u32*)sc.size.p,
-                                   (u32*)sc.aux.p, status, (u32*)sc.ioff.p, (u32*)sc.nn.p, pend1, counters + 4, pend2, counters + 8, e->sm_count, nullptr, nullptr, -1);
-      if (prof) prof_mark(e, st, &c0);
-      if (e->spread_min) {
-        // the per-thread list, split: small items 32 to a warp, large ones a warp each (k_spread)
-        size_t max_big = (size_t)(in_bytes / e->spread_min) + 1;  // items of at least spread_min bytes
-        if (max_big > GGR_SPREAD_CAP) max_big = GGR_SPREAD_CAP;
-        if (!ensure(e, sc.spread, (max_big * 32 + (size_t)n) * 4 + 64)) return GGR_ERR_CUDA;
-        u32* sp_cnt = (u32*)sc.spread.p;
-        u32* sp_list = sp_cnt + 16;
-        u32* sp_small = sp_list + max_big * 32;
-        if (!cuda_ok(e, cudaMemsetAsync(sp_cnt, 0, 64, st), "memset") || !cuda_ok(e, cudaMemsetAsync(sp_list, 0xFF, max_big * 32 * 4, st), "memset"))
-          return GGR_ERR_CUDA;
-        for (int phase = 0; phase < 2; phase++)
-          k_spread<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(phase, n, in_off, e->spread_min, pend2, counters + 8, nullptr, sp_small, sp_list, sp_cnt, (u32)max_big);
-        ggr_launch_encode_parse(st, (unsigned)((max_big * 32 + GGR_BLOCK - 1) / GGR_BLOCK), s->d_blob, n, n_msgs, msg_id, in, in_off, (u8*)sc.ir.p,
-                                (u32*)sc.size.p, (u32*)sc.aux.p, status, (u64*)sc.sums.p, sp_list, sp_cnt);
-        ggr_launch_encode_parse(st, (unsigned)nb, s->d_blob, n, n_msgs, msg_id, in, in_off, (u8*)sc.ir.p, (u32*)sc.size.p,
-                                (u32*)sc.aux.p, status, (u64*)sc.sums.p, sp_small, sp_cnt + 1);
-        e->launches += 3;
-      } else {
-        ggr_launch_encode_parse(st, (unsigned)nb, s->d_blob, n, n_msgs, msg_id, in, in_off, (u8*)sc.ir.p, (u32*)sc.size.p,
-                                (u32*)sc.aux.p, status, (u64*)sc.sums.p, pend2, counters + 8);
-      }
-      if (prof) prof_mark(e, st, &c1);
-      if (frame) ggr_launch_frame_sizes(st, n, (u32*)sc.size.p, status);
-      ggr_launch_block_sums(st, (unsigned)nb, n, (const u32*)sc.size.p, (u64*)sc.sums.p);
-      if (prof) {
-        e->spans.push_back({11, m0, t_tok});  // router + token index
-        e->spans.push_back({8, t1, c0});    // walker, tier 2
-        e->spans.push_back({0, c0, c1});
-        prof_mark(e, st, &m1);
-        e->spans.push_back({9, c1, m1});
-      }
-      e->launches += e->use_walk ? 8 : 5;  // + the token-index kernel of tier 1 (+ the place kernel of the token-parallel walker)
-    } else {
-      ggr_launch_encode_parse(st, (unsigned)nb, s->d_blob, n, n_msgs, msg_id, in, in_off, (u8*)sc.ir.p, (u32*)sc.size.p,
-                              (u32*)sc.aux.p, status, (u64*)sc.sums.p, nullptr, nullptr);
-      if (frame) {
-        ggr_launch_frame_sizes(st, n, (u32*)sc.size.p, status);
-        ggr_launch_block_sums(st, (unsigned)nb, n, (const u32*)sc.size.p, (u64*)sc.sums.p);
-      }
-      if (prof) prof_mark(e, st, &m1);
-    }
-    k_scan_blocks<<<1, 1024, 0, st>>>((u64*)sc.sums.p, nb, out_off + n);
-    if (prof) prof_mark(e, st, &m2);
-    ggr_launch_encode_emit(st, (unsigned)nb, n, in, in_off, (const u8*)sc.ir.p, (const u32*)sc.size.p,
-                           (const u32*)sc.aux.p, status, (const u64*)sc.sums.p, out, out_cap, out_off,
-                           e->use_coop_enc ? (const u32*)sc.nn.p : nullptr, frame);
-    if (e->use_coop_enc) {
-      size_t x1 = 0;
-      if (prof) {
-        prof_mark(e, st, &mx);
-        have_mx = true;
-      }
-      ggr_launch_encode_coop_emit(st, n, in, in_off, (const u8*)sc.ir.p, (const u32*)sc.ioff.p, (const u32*)sc.nn.p,
-                                  (const u32*)sc.size.p, status, out, out_off, e->sm_count, (const u32*)sc.pend.p + 32,
-                                  (const u32*)sc.pend.p, frame);
-      if (prof) {
-        prof_mark(e, st, &x1);
-        e->spans.push_back({10, mx, x1});
-      }
-      e->launches += 1;
-    }
-  } else {
-    // Reply side: the warp-cooperative kernels take every regular item; the per-thread kernels
-    // then walk only what was left pending (irregular field order, maps, malformed wire, ...).
-    const bool coop = e->use_coop;
-    size_t c0 = 0, c1 = 0;
-    // a map entry takes at least 4 bytes of wire; both passes sort, the fast walk may give way to the slow one
-    const uint64_t want_recs = in_bytes / 4 * 3 + 1024;
-    const uint32_t sort_cap = (uint32_t)(want_recs > 0x3FFFFFFFull ? 0x3FFFFFFFull : want_recs);
-    if (!ensure(e, sc.sortpool, (size_t)sort_cap * 16 + 16)) return GGR_ERR_CUDA;
-    if (!cuda_ok(e, cudaMemsetAsync(sc.sortpool.p, 0, 16, st), "memset")) return GGR_ERR_CUDA;
-    if (coop) {
-      // second tier's tables: a field occurrence takes at least 2 bytes of wire; the pool is capped at 4 M entries (128 MB)
-      const uint64_t want_ent = in_bytes / 2 + 4096;
-      const uint32_t pool_cap = (uint32_t)(want_ent > (4ull << 20) ? (4ull << 20) : want_ent);
-      if (!ensure(e, sc.ir, ggr_decode_coop_table_bytes(n)) || !ensure(e, sc.nn, (size_t)n * 4) ||
-          !ensure(e, sc.pend, (size_t)n * 8 + 64) || !ensure(e, sc.tabpool, (size_t)pool_cap * 32 + 32) || !ensure(e, sc.taboff, (size_t)n * 4))
-        return GGR_ERR_CUDA;
-      u32* counters = (u32*)sc.pend.p;
-      u32* big = counters + 16;
-      if (!cuda_ok(e, cudaMemsetAsync(counters, 0, 64, st), "memset") || !cuda_ok(e, cudaMemsetAsync(sc.tabpool.p, 0, 32, st), "memset")) return GGR_ERR_CUDA;
-      k_route<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(n, in_off, e->min_wire, 0x3FFFFF00u, big, counters, nullptr, nullptr, (u32*)sc.aux.p);
-      ggr_launch_decode_coop_size(st, n, s->d_blob, n_msgs, msg_id, in, in_off, flags, (u32*)sc.size.p, (u32*)sc.aux.p, status,
-                                  sc.ir.p, (u32*)sc.nn.p, e->sm_count, big, counters, big + n, counters + 4, sc.tabpool.p, pool_cap, (u32*)sc.taboff.p);
-      if (prof) {
-        prof_mark(e, st, &c0);
-        e->spans.push_back({6, m0, c0});
-        m0 = c0;
-      }
-    }
-    // large items the warp-cooperative kernels left: a warp each (k_spread), sized before and written after the pass over the batch
-    const bool spread = coop && e->spread_min != 0;
-    size_t max_big = spread ? (size_t)(in_bytes / e->spread_min) + 1 : 0;
-    if (max_big > GGR_SPREAD_CAP) max_big = GGR_SPREAD_CAP;
-    u32* sp_cnt = nullptr;
-    if (spread) {
-      if (!ensure(e, sc.spread, max_big * 32 * 4 + 64)) return GGR_ERR_CUDA;
-      sp_cnt = (u32*)sc.spread.p;
-      if (!cuda_ok(e, cudaMemsetAsync(sp_cnt, 0, 64, st), "memset") || !cuda_ok(e, cudaMemsetAsync(sp_cnt + 16, 0xFF, max_big * 32 * 4, st), "memset"))
-        return GGR_ERR_CUDA;
-      for (int phase = 0; phase < 2; phase++)
-        k_spread<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(phase, n, in_off, e->spread_min, nullptr, nullptr, (const u32*)sc.aux.p, nullptr, sp_cnt + 16, sp_cnt, (u32)max_big);
-      ggr_launch_decode_size(st, (unsigned)((max_big * 32 + GGR_BLOCK - 1) / GGR_BLOCK), s->d_blob, n, n_msgs, msg_id, in, in_off, flags,
-                             (u32*)sc.size.p, (u32*)sc.aux.p, status, (u64*)sc.sums.p, 1, sc.sortpool.p, sort_cap, sp_cnt + 16, sp_cnt);
-      e->launches += 4;
-    }
-    ggr_launch_decode_size(st, (unsigned)nb, s->d_blob, n, n_msgs, msg_id, in, in_off, flags, (u32*)sc.size.p,
-                           (u32*)sc.aux.p, status, (u64*)sc.sums.p, coop ? 1 : 0, sc.sortpool.p, sort_cap);
-    if (prof) prof_mark(e, st, &m1);
-    k_scan_blocks<<<1, 1024, 0, st>>>((u64*)sc.sums.p, nb, out_off + n);
-    if (prof) prof_mark(e, st, &m2);
-    ggr_launch_decode_write(st, (unsigned)nb, s->d_blob, n, msg_id, in, in_off, flags, (const u32*)sc.size.p,
-                            (const u32*)sc.aux.p, status, (const u64*)sc.sums.p, out, out_cap, out_off, sc.sortpool.p, sort_cap);
-    if (spread)
-      ggr_launch_decode_write(st, (unsigned)((max_big * 32 + GGR_BLOCK - 1) / GGR_BLOCK), s->d_blob, n, msg_id, in, in_off, flags,
-                              (const u32*)sc.size.p, (const u32*)sc.aux.p, status, (const u64*)sc.sums.p, out, out_cap, out_off, sc.sortpool.p,
-                              sort_cap, sp_cnt + 16, sp_cnt);
-    if (coop) {
-      if (prof) prof_mark(e, st, &c1);
-      ggr_launch_decode_coop_write(st, n, s->d_blob, in, in_off, flags, (const u32*)sc.size.p, (const u32*)sc.aux.p, status, sc.ir.p,
-                                   (const u32*)sc.nn.p, out, out_off, e->sm_count, (const u32*)sc.pend.p + 16, (const u32*)sc.pend.p, sc.tabpool.p,
-                                   (const u32*)sc.taboff.p);
-      if (prof) {
-        prof_mark(e, st, &m3);
-        e->spans.push_back({3, m0, m1});
-        e->spans.push_back({4, m1, m2});
-        e->spans.push_back({5, m2, c1});
-        e->spans.push_back({7, c1, m3});
-      }
-      e->launches += 7;
-      return cuda_ok(e, cudaGetLastError(), "kernel launch") ? GGR_SUCCESS : GGR_ERR_CUDA;
-    }
-  }
-  if (prof) {
-    prof_mark(e, st, &m3);
-    int base = encode ? 0 : 3;
-    if (!(encode && e->use_coop_enc)) e->spans.push_back({base + 0, m0, m1});
-    e->spans.push_back({base + 1, m1, m2});
-    e->spans.push_back({base + 2, m2, have_mx ? mx : m3});
-  }
-  e->launches += 3;
-  return cuda_ok(e, cudaGetLastError(), "kernel launch") ? GGR_SUCCESS : GGR_ERR_CUDA;
 }
 
 // One failing request item through the per-thread parser again (the kernel that owns the request-side semantics),
@@ -877,7 +911,7 @@ int ggr_encode_diagnose(ggr_engine* e, const ggr_schema* s, int32_t msg_id, cons
   std::lock_guard<std::mutex> g(e->mu);
   DeviceGuard dg(e->device);
   const size_t in_cap = ((size_t)json_len + 15) / 16 * 16 + 64;
-  const size_t ir_bytes = (size_t)json_len * 8 + 128 + 256;
+  const size_t ir_bytes = ggr_ir_bytes(json_len, 1);
   // one allocation: input | offsets | message id | size, first, status, error position | block sums | IR
   const size_t o_off = in_cap, o_msg = o_off + 16, o_res = o_msg + 16, o_sums = o_res + 16, o_ir = o_sums + 16;
   uint8_t* d = nullptr;
@@ -962,39 +996,32 @@ int ggr_decode_batch_dev(ggr_engine* e, const ggr_schema* s, int64_t n, const in
 static int run_request_dev(ggr_engine* e, const ggr_schema* s, Scratch& sc, int64_t n, const uint8_t* in, const uint64_t* in_off,
                            uint64_t in_bytes, uint8_t* out, uint64_t out_cap, uint64_t* out_off, int32_t* method, uint32_t* id_span,
                            int32_t* status, cudaStream_t st) {
-  if (!e || !s || n < 0 || (n > 0 && (!in || !in_off || !out_off || !status || !method || !id_span))) return GGR_ERR_INVALID_ARGUMENT;
-  if (((uintptr_t)in & 15) || ((uintptr_t)out & 7)) return GGR_ERR_INVALID_ARGUMENT;
-  DeviceGuard dg(e->device);
-  if (n == 0) return cuda_ok(e, cudaMemsetAsync(out_off, 0, sizeof(uint64_t), st), "memset") ? GGR_SUCCESS : GGR_ERR_CUDA;
-  const long long nb = (n + GGR_BLOCK - 1) / GGR_BLOCK;
-  if (!ensure(e, sc.size, (size_t)n * 4) || !ensure(e, sc.aux, (size_t)n * 4) || !ensure(e, sc.sums, (size_t)nb * 8) ||
-      !ensure(e, sc.ir, (size_t)in_bytes * 8 + (size_t)n * 128 + 256) || !ensure(e, sc.pend, (size_t)n * 12 + 64) ||
-      !ensure(e, sc.ioff, (size_t)in_bytes * 2 + (size_t)n * 32 + 64) || !ensure(e, sc.nn, (size_t)n * 4))
-    return GGR_ERR_CUDA;
-  u32* counters = (u32*)sc.pend.p;
-  u32* big = counters + 16;
-  u32* pend1 = big + n;
-  u32* rest = pend1 + n;
-  if (!cuda_ok(e, cudaMemsetAsync(counters, 0, 64, st), "memset") || !cuda_ok(e, cudaMemsetAsync(sc.nn.p, 0, (size_t)n * 4, st), "memset"))
-    return GGR_ERR_CUDA;
-  const u32 n_msgs = (u32)s->cs.msg_names.size();
-  // bodies above the parser's input limit cannot be taken
-  k_route<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(n, in_off, 0u, 65000u - 16u, big, counters, rest, counters + 8, nullptr);
-  ggr_launch_encode_coop_tok(st, n, in, in_off, (u8*)sc.ir.p, big, counters, e->sm_count);
-  ggr_launch_encode_coop_parse(st, 0, n, s->d_blob, n_msgs, nullptr, in, in_off, (u8*)sc.ir.p, (u32*)sc.size.p, (u32*)sc.aux.p, status,
-                               (u32*)sc.ioff.p, (u32*)sc.nn.p, big, counters, pend1, counters + 4, e->sm_count, method, id_span, -1);
-  ggr_launch_encode_coop_parse(st, 1, n, s->d_blob, n_msgs, nullptr, in, in_off, (u8*)sc.ir.p, (u32*)sc.size.p, (u32*)sc.aux.p, status,
-                               (u32*)sc.ioff.p, (u32*)sc.nn.p, pend1, counters + 4, rest, counters + 8, e->sm_count, method, id_span,
-                               GGR_ST_UNSUPPORTED);
-  k_mark<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(rest, counters + 8, status, (u32*)sc.size.p, (u32*)sc.aux.p, GGR_ST_UNSUPPORTED);
-  ggr_launch_block_sums(st, (unsigned)nb, n, (const u32*)sc.size.p, (u64*)sc.sums.p);
-  k_scan_blocks<<<1, 1024, 0, st>>>((u64*)sc.sums.p, nb, out_off + n);
-  ggr_launch_encode_emit(st, (unsigned)nb, n, in, in_off, (const u8*)sc.ir.p, (const u32*)sc.size.p, (const u32*)sc.aux.p, status,
-                         (const u64*)sc.sums.p, out, out_cap, out_off, (const u32*)sc.nn.p, 0);
-  ggr_launch_encode_coop_emit(st, n, in, in_off, (const u8*)sc.ir.p, (const u32*)sc.ioff.p, (const u32*)sc.nn.p, (const u32*)sc.size.p,
-                              status, out, out_off, e->sm_count, big, counters, 0);
-  e->launches += 9;
-  return cuda_ok(e, cudaGetLastError(), "kernel launch") ? GGR_SUCCESS : GGR_ERR_CUDA;
+  const bool have_args = in && in_off && out_off && status && method && id_span;
+  return run_batch(e, s, sc, n, have_args, in, out, out_off, st, [&](long long nb) {
+    BodyLists L;
+    if (!ensure(e, sc.ir, ggr_ir_bytes(in_bytes, n)) || !ensure(e, sc.ioff, ggr_ioff_bytes(in_bytes, n)) || !ensure(e, sc.nn, (size_t)n * 4) ||
+        !make_lists(e, sc.pend, n, st, &L) || !cuda_ok(e, cudaMemsetAsync(sc.nn.p, 0, (size_t)n * 4, st), "memset"))
+      return GGR_ERR_CUDA;
+    const u32 n_msgs = (u32)s->cs.msg_names.size();
+    u8* ir = (u8*)sc.ir.p;
+    u32 *size = (u32*)sc.size.p, *first = (u32*)sc.aux.p, *ioff = (u32*)sc.ioff.p, *nn = (u32*)sc.nn.p;
+    u64* sums = (u64*)sc.sums.p;
+    // bodies above the parser's input limit cannot be taken
+    k_route<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(n, in_off, 0u, 65000u - 16u, L.lockstep.item, &L.lockstep.h->n, L.rest.item,
+                                                        &L.rest.h->n, nullptr);
+    ggr_launch_encode_coop_tok(st, n, in, in_off, ir, L.lockstep.item, L.lockstep.h, e->sm_count);
+    ggr_launch_encode_coop_parse(st, 0, n, s->d_blob, n_msgs, nullptr, in, in_off, ir, size, first, status, ioff, nn, L.lockstep.item,
+                                 L.lockstep.h, L.tier1_left.item, L.tier1_left.h, e->sm_count, method, id_span, -1);
+    ggr_launch_encode_coop_parse(st, 1, n, s->d_blob, n_msgs, nullptr, in, in_off, ir, size, first, status, ioff, nn, L.tier1_left.item,
+                                 L.tier1_left.h, L.rest.item, L.rest.h, e->sm_count, method, id_span, GGR_ST_UNSUPPORTED);
+    k_mark<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(L.rest.item, &L.rest.h->n, status, size, first, GGR_ST_UNSUPPORTED);
+    ggr_launch_block_sums(st, (unsigned)nb, n, size, sums);
+    k_scan_blocks<<<1, 1024, 0, st>>>(sums, nb, out_off + n);
+    ggr_launch_encode_emit(st, (unsigned)nb, n, in, in_off, ir, size, first, status, sums, out, out_cap, out_off, nn, 0);
+    ggr_launch_encode_coop_emit(st, n, in, in_off, ir, ioff, nn, size, status, out, out_off, e->sm_count, L.lockstep.item, L.lockstep.h, 0);
+    e->launches += 9;
+    return GGR_SUCCESS;
+  });
 }
 
 // Reply half + result wrapping on device buffers: decode into scratch texts, size the bodies, scan,

@@ -18,7 +18,7 @@ __global__ void __launch_bounds__(WARPS * 32)
 k_decode_coop_size(const u8* __restrict__ blob, long long n, u32 n_msgs, const i32* __restrict__ msg_id,
                    const u8* __restrict__ in, const u64* __restrict__ in_off, u32 flags, u32* __restrict__ size,
                    u32* __restrict__ mode, i32* __restrict__ status, U4* __restrict__ tab, u32* __restrict__ nent,
-                   const u32* __restrict__ list, const u32* __restrict__ list_n, u32* __restrict__ pending, u32* __restrict__ n_pending,
+                   const u32* __restrict__ list, const GgrList* __restrict__ list_h, u32* __restrict__ pending, GgrList* __restrict__ pending_h,
                    U4* __restrict__ pool, u32 pool_cap, u32* __restrict__ tab_off) {
   extern __shared__ __align__(16) unsigned char smem[];
   SH* S = reinterpret_cast<SH*>(smem);
@@ -27,8 +27,8 @@ k_decode_coop_size(const u8* __restrict__ blob, long long n, u32 n_msgs, const i
   cx.T = ggr_tables(blob);
   cx.flags = flags;
   // the items of `list` (the router's choice: not too small, not too large); mode[] is PENDING for all others
-  const long long total = (long long)*list_n;
-  u32* ticket = const_cast<u32*>(list_n) + 1;  // zeroed with the list length; +2 is the write kernel's
+  const long long total = (long long)list_h->n;
+  u32* ticket = const_cast<u32*>(&list_h->tok_ticket);
   // two tickets in flight: the wire bytes of the item after the current one are asked for in L2 (bulk prefetch)
   u32 drawn = wp_ticket_draw(ticket);
   long long slot = wp_ticket_take(drawn);
@@ -71,7 +71,7 @@ k_decode_coop_size(const u8* __restrict__ blob, long long n, u32 n_msgs, const i
       } else {
         mode[item] = GGR_MODE_PENDING;
         nent[item] = 0;
-        if (pending) pending[atomicAdd(n_pending, 1u)] = (u32)item;
+        if (pending) pending[atomicAdd(&pending_h->n, 1u)] = (u32)item;
       }
     }
     slot = next;
@@ -84,7 +84,7 @@ __global__ void __launch_bounds__(COOP_WRITE_WARPS * 32, COOP_WRITE_MINB)
 k_decode_coop_write(const u8* __restrict__ blob, long long n, const u8* __restrict__ in, const u64* __restrict__ in_off,
                     u32 flags, const u32* __restrict__ size, const u32* __restrict__ mode, i32* __restrict__ status,
                     const U4* __restrict__ tab, const u32* __restrict__ nent, u8* __restrict__ out,
-                    const u64* __restrict__ out_off, const u32* __restrict__ list, const u32* __restrict__ list_n,
+                    const u64* __restrict__ out_off, const u32* __restrict__ list, const GgrList* __restrict__ list_h,
                     const U4* __restrict__ pool, const u32* __restrict__ tab_off) {
   extern __shared__ __align__(16) unsigned char smem[];
   CoopStage* E = reinterpret_cast<CoopStage*>(smem);
@@ -92,8 +92,8 @@ k_decode_coop_write(const u8* __restrict__ blob, long long n, const u8* __restri
   DecCtx cx;
   cx.T = ggr_tables(blob);
   cx.flags = flags;
-  const long long total = (long long)*list_n;
-  u32* ticket = const_cast<u32*>(list_n) + 2;
+  const long long total = (long long)list_h->n;
+  u32* ticket = const_cast<u32*>(&list_h->item_ticket);
   u32 drawn = wp_ticket_draw(ticket);
   long long slot = wp_ticket_take(drawn);
   drawn = wp_ticket_draw(ticket);
@@ -131,40 +131,27 @@ int ggr_decode_coop_init() {
                                        (int)(sizeof(CoopStage) * COOP_WRITE_WARPS));
   return (a == cudaSuccess && b == cudaSuccess) ? 0 : -1;
 }
-template <class SH>
-static unsigned coop_grid(long long n, int sm_count) {
-  // resident blocks per SM: what the entry tables in shared memory allow (6 with 224 entries per warp, 4 with 320)
-  static int per_sm = 0;
-  if (per_sm == 0 &&
-      (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_decode_coop_size<SH, COOP_WARPS>, COOP_WARPS * 32, coop_smem_bytes<SH, COOP_WARPS>()) != cudaSuccess ||
-       per_sm < 1))
-    per_sm = 4;
-  long long want = (n + COOP_WARPS - 1) / COOP_WARPS, cap = (long long)sm_count * per_sm;
-  return (unsigned)(want < cap ? want : cap);
-}
-
 void ggr_launch_decode_coop_size(cudaStream_t st, long long n, const uint8_t* blob, uint32_t n_msgs, const int32_t* msg_id,
                                  const uint8_t* in, const uint64_t* in_off, uint32_t flags, uint32_t* size, uint32_t* mode,
                                  int32_t* status, void* tab, uint32_t* nent, int sm_count, const uint32_t* list,
-                                 const uint32_t* list_n, uint32_t* pending, uint32_t* n_pending, void* pool, uint32_t pool_cap,
+                                 const GgrList* list_h, uint32_t* pending, GgrList* pending_h, void* pool, uint32_t pool_cap,
                                  uint32_t* tab_off) {
   // first tier over the router's list; second tier (tables of thousands of entries, one warp per SM, saved in the pool; its
-  // list length lives on the device) over what the first left
-  k_decode_coop_size<CoopShared, COOP_WARPS><<<coop_grid<CoopShared>(n, sm_count), COOP_WARPS * 32, coop_smem_bytes<CoopShared, COOP_WARPS>(), st>>>(
-      blob, n, n_msgs, msg_id, in, (const u64*)in_off, flags, size, mode, status, (U4*)tab, nent, list, list_n, pending, n_pending, nullptr, 0u, nullptr);
+  // list length lives on the device) over what the first left.  Resident blocks of the first tier: what the entry tables
+  // in shared memory allow (6 with 224 entries per warp, 4 with 320)
+  static const int resident = ggr_resident_blocks((const void*)k_decode_coop_size<CoopShared, COOP_WARPS>, COOP_WARPS * 32,
+                                                  coop_smem_bytes<CoopShared, COOP_WARPS>(), 4);
+  k_decode_coop_size<CoopShared, COOP_WARPS><<<ggr_persistent_grid(n, COOP_WARPS, sm_count, resident), COOP_WARPS * 32, coop_smem_bytes<CoopShared, COOP_WARPS>(), st>>>(
+      blob, n, n_msgs, msg_id, in, (const u64*)in_off, flags, size, mode, status, (U4*)tab, nent, list, list_h, pending, pending_h, nullptr, 0u, nullptr);
   k_decode_coop_size<CoopSharedBig, 1><<<(unsigned)sm_count, 32, coop_smem_bytes<CoopSharedBig, 1>(), st>>>(
-      blob, n, n_msgs, msg_id, in, (const u64*)in_off, flags, size, mode, status, (U4*)tab, nent, pending, n_pending, nullptr, nullptr, (U4*)pool, pool_cap,
+      blob, n, n_msgs, msg_id, in, (const u64*)in_off, flags, size, mode, status, (U4*)tab, nent, pending, pending_h, nullptr, nullptr, (U4*)pool, pool_cap,
       tab_off);
 }
 void ggr_launch_decode_coop_write(cudaStream_t st, long long n, const uint8_t* blob, const uint8_t* in, const uint64_t* in_off,
                                   uint32_t flags, const uint32_t* size, const uint32_t* mode, int32_t* status, const void* tab,
                                   const uint32_t* nent, uint8_t* out, const uint64_t* out_off, int sm_count,
-                                  const uint32_t* list, const uint32_t* list_n, const void* pool, const uint32_t* tab_off) {
-  static int per_sm = 0;
-  if (per_sm == 0 && (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_decode_coop_write, COOP_WRITE_WARPS * 32, sizeof(CoopStage) * COOP_WRITE_WARPS) != cudaSuccess || per_sm < 1))
-    per_sm = 6;
-  long long want = (n + COOP_WRITE_WARPS - 1) / COOP_WRITE_WARPS, cap = (long long)sm_count * per_sm;
-  unsigned nb = (unsigned)(want < cap ? want : cap);
-  k_decode_coop_write<<<nb, COOP_WRITE_WARPS * 32, sizeof(CoopStage) * COOP_WRITE_WARPS, st>>>(
-      blob, n, in, (const u64*)in_off, flags, size, mode, status, (const U4*)tab, nent, out, (const u64*)out_off, list, list_n, (const U4*)pool, tab_off);
+                                  const uint32_t* list, const GgrList* list_h, const void* pool, const uint32_t* tab_off) {
+  static const int resident = ggr_resident_blocks((const void*)k_decode_coop_write, COOP_WRITE_WARPS * 32, sizeof(CoopStage) * COOP_WRITE_WARPS, 6);
+  k_decode_coop_write<<<ggr_persistent_grid(n, COOP_WRITE_WARPS, sm_count, resident), COOP_WRITE_WARPS * 32, sizeof(CoopStage) * COOP_WRITE_WARPS, st>>>(
+      blob, n, in, (const u64*)in_off, flags, size, mode, status, (const U4*)tab, nent, out, (const u64*)out_off, list, list_h, (const U4*)pool, tab_off);
 }

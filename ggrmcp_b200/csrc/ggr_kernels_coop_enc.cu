@@ -14,18 +14,16 @@
 #define CE_TOK_BLOCKS 7
 __global__ void __launch_bounds__(CE_WARPS * 32, CE_TOK_BLOCKS)
 k_encode_coop_tok(long long n, const u8* __restrict__ in, const u64* __restrict__ in_off, u8* __restrict__ ir,
-                  const u32* __restrict__ list, const u32* __restrict__ list_n) {
+                  const u32* __restrict__ list, const GgrList* __restrict__ list_h) {
   extern __shared__ __align__(16) unsigned char smem[];
   CeLut& lut = *reinterpret_cast<CeLut*>(smem);
   CoopTok* S = reinterpret_cast<CoopTok*>(smem + ((sizeof(CeLut) + 15) & ~(size_t)15));
   const u32 warp = threadIdx.x >> 5;
   ce_lut_init(lut, threadIdx.x, CE_WARPS * 32);
   __syncthreads();
-  const long long total = list ? (long long)*list_n : n;
+  const long long total = list ? (long long)list_h->n : n;
   const u64 a0 = in_off[0];
-  // the words after a list's length are zeroed with it and serve as ticket counters: +1 this kernel,
-  // +2 the walker
-  u32* ticket = list ? const_cast<u32*>(list_n) + 1 : nullptr;
+  u32* ticket = list ? const_cast<u32*>(&list_h->tok_ticket) : nullptr;
   const long long stride = ticket ? 0 : (long long)gridDim.x * CE_WARPS;
   u32 drawn = ticket ? wp_ticket_draw(ticket) : 0u;
   for (long long slot = ticket ? wp_ticket_take(drawn) : (long long)blockIdx.x * CE_WARPS + warp; slot < total;
@@ -34,10 +32,9 @@ k_encode_coop_tok(long long n, const u8* __restrict__ in, const u64* __restrict_
     const long long item = list ? (long long)list[slot] : slot;
     const u64 a = in_off[item], b = in_off[item + 1];
     if (b < a || b - a > (u64)CE_MAX_INPUT - 16u) continue;
-    const u64 node_off = ((a - a0) >> 1) + 8ull * (u64)item;
-    const u32 cap = (u32)((((b - a0) >> 1) + 8ull * (u64)(item + 1)) - node_off);
+    const GgrRegion r = ggr_item_region(a0, a, b, (u64)item);
     const u32 s0 = (u32)(a & 15ull);
-    ce_tok_item(S[warp], lut, in + (a & ~15ull), s0, s0 + (u32)(b - a), ir + node_off * 16, cap);
+    ce_tok_item(S[warp], lut, in + (a & ~15ull), s0, s0 + (u32)(b - a), ir + r.node_off * 16, r.cap);
   }
 }
 
@@ -49,8 +46,8 @@ __global__ void __launch_bounds__(CE_WARPS * 32)
 k_encode_coop_parse(const u8* __restrict__ blob, long long n, u32 n_msgs, const i32* __restrict__ msg_id,
                     const u8* __restrict__ in, const u64* __restrict__ in_off, u8* __restrict__ ir, u32* __restrict__ size,
                     u32* __restrict__ first, i32* __restrict__ status, u32* __restrict__ ioff, u32* __restrict__ nnodes,
-                    const u32* __restrict__ list, const u32* __restrict__ list_n, u32* __restrict__ pending,
-                    u32* __restrict__ n_pending, i32* __restrict__ method, u32* __restrict__ id_span, i32 final_status) {
+                    const u32* __restrict__ list, const GgrList* __restrict__ list_h, u32* __restrict__ pending,
+                    GgrList* __restrict__ pending_h, i32* __restrict__ method, u32* __restrict__ id_span, i32 final_status) {
   extern __shared__ __align__(16) unsigned char smem[];
   CeLut& lut = *reinterpret_cast<CeLut*>(smem);
   SH* S = reinterpret_cast<SH*>(smem + ((sizeof(CeLut) + 15) & ~(size_t)15));
@@ -58,10 +55,10 @@ k_encode_coop_parse(const u8* __restrict__ blob, long long n, u32 n_msgs, const 
   ce_lut_init(lut, threadIdx.x, CE_WARPS * 32);
   __syncthreads();
   // persistent warps: warp w of block b takes slots b * CE_WARPS + w, + gridDim.x * CE_WARPS, ...
-  const long long total = list ? (long long)*list_n : n;
+  const long long total = list ? (long long)list_h->n : n;
   const Tables T = ggr_tables(blob);
   const u64 a0 = in_off[0];  // IR regions are laid out relative to the first offset of the batch
-  u32* ticket = list ? const_cast<u32*>(list_n) + 2 : nullptr;
+  u32* ticket = list ? const_cast<u32*>(&list_h->item_ticket) : nullptr;
   const long long stride = ticket ? 0 : (long long)gridDim.x * CE_WARPS;
   u32 drawn = ticket ? wp_ticket_draw(ticket) : 0u;
   for (long long slot = ticket ? wp_ticket_take(drawn) : (long long)blockIdx.x * CE_WARPS + warp; slot < total;
@@ -78,11 +75,10 @@ k_encode_coop_parse(const u8* __restrict__ blob, long long n, u32 n_msgs, const 
     res.first = GGR_NIL;
     res.n_nodes = 0;
     if (m >= 0 && (u32)m < n_msgs && b >= a && b - a <= (u64)CE_MAX_INPUT - 16u) {
-      const u64 node_off = ((a - a0) >> 1) + 8ull * (u64)item;
-      const u32 cap = (u32)((((b - a0) >> 1) + 8ull * (u64)(item + 1)) - node_off);
+      const GgrRegion r = ggr_item_region(a0, a, b, (u64)item);
       const u8* base = in + (a & ~15ull);
       const u32 s0 = (u32)(a & 15ull);
-      ok = ce_parse_item<SH, ENV, PRE>(S[warp], lut, T, (u32)m, base, s0, s0 + (u32)(b - a), ir + node_off * 16, ioff + node_off, cap, &res);
+      ok = ce_parse_item<SH, ENV, PRE>(S[warp], lut, T, (u32)m, base, s0, s0 + (u32)(b - a), ir + r.node_off * 16, ioff + r.node_off, r.cap, &res);
     }
     if (lane == 0) {
       if (ok) {
@@ -100,7 +96,7 @@ k_encode_coop_parse(const u8* __restrict__ blob, long long n, u32 n_msgs, const 
         nnodes[item] = 0;
         first[item] = GGR_NIL;
         if (final_status >= 0) status[item] = final_status;  // last tier of the envelope mode: no per-thread path
-        else pending[atomicAdd(n_pending, 1u)] = (u32)item;
+        else pending[atomicAdd(&pending_h->n, 1u)] = (u32)item;
       }
     }
   }
@@ -112,12 +108,12 @@ __global__ void __launch_bounds__(CE_WARPS * 32)
 k_encode_coop_emit(long long n, const u8* __restrict__ in, const u64* __restrict__ in_off, const u8* __restrict__ ir,
                    const u32* __restrict__ ioff, const u32* __restrict__ nnodes, const u32* __restrict__ size,
                    const i32* __restrict__ status, u8* __restrict__ out, const u64* __restrict__ out_off,
-                   const u32* __restrict__ list, const u32* __restrict__ list_n, u32 frame) {
+                   const u32* __restrict__ list, const GgrList* __restrict__ list_h, u32 frame) {
   extern __shared__ __align__(16) unsigned char smem[];
   CoopEmit* E = reinterpret_cast<CoopEmit*>(smem);
   const u32 warp = threadIdx.x >> 5;
   const u64 a0 = in_off[0];
-  const long long total = (long long)*list_n;  // the router's lock-step items
+  const long long total = (long long)list_h->n;  // the router's lock-step items
   // fixed stride here: an item takes a few microseconds, and tickets for a whole batch of them in a millisecond
   // would run into the rate of atomics on one address
   for (long long slot = (long long)blockIdx.x * CE_WARPS + warp; slot < total; slot += (long long)gridDim.x * CE_WARPS) {
@@ -127,7 +123,7 @@ k_encode_coop_emit(long long n, const u8* __restrict__ in, const u64* __restrict
     const u32 sz = size[item];
     if (nn <= 1 || sz <= frame || status[item] != GST_OK) continue;
     const u64 a = in_off[item], b = in_off[item + 1];
-    const u64 node_off = ((a - a0) >> 1) + 8ull * (u64)item + (u64)(nw >> 16);
+    const u64 node_off = ggr_item_region(a0, a, b, (u64)item).node_off + (u64)(nw >> 16);
     // frame: the 5-byte message header in front of the payload was written by k_encode_emit
     ce_emit_item(E[warp], in + (a & ~15ull), (u32)(a & 15ull) + (u32)(b - a), ir + node_off * 16, ioff + node_off, nn,
                  out + out_off[item] + frame, sz - frame);
@@ -157,50 +153,45 @@ int ggr_encode_coop_init() {
 template <class SH, bool ENV, bool PRE>
 static void ce_launch(cudaStream_t st, unsigned nb, long long n, const uint8_t* blob, uint32_t n_msgs, const int32_t* msg_id,
                       const uint8_t* in, const uint64_t* in_off, uint8_t* ir, uint32_t* size, uint32_t* first, int32_t* status,
-                      uint32_t* ioff, uint32_t* nnodes, const uint32_t* list, const uint32_t* list_n, uint32_t* pending,
-                      uint32_t* n_pending, int32_t* method, uint32_t* id_span, int32_t final_status) {
+                      uint32_t* ioff, uint32_t* nnodes, const uint32_t* list, const GgrList* list_h, uint32_t* pending,
+                      GgrList* pending_h, int32_t* method, uint32_t* id_span, int32_t final_status) {
   k_encode_coop_parse<SH, ENV, PRE><<<nb, CE_WARPS * 32, ce_smem_bytes<SH>(), st>>>(
-      blob, n, n_msgs, msg_id, in, (const u64*)in_off, ir, size, first, status, ioff, nnodes, list, list_n, pending, n_pending, method,
+      blob, n, n_msgs, msg_id, in, (const u64*)in_off, ir, size, first, status, ioff, nnodes, list, list_h, pending, pending_h, method,
       id_span, final_status);
 }
 
 // token index of tier 1 (before ggr_launch_encode_coop_parse with tier 0, same list)
 void ggr_launch_encode_coop_tok(cudaStream_t st, long long n, const uint8_t* in, const uint64_t* in_off, uint8_t* ir,
-                                const uint32_t* list, const uint32_t* list_n, int sm_count) {
-  const long long want = (n + CE_WARPS - 1) / CE_WARPS, cap_t = (long long)sm_count * CE_TOK_BLOCKS;
-  k_encode_coop_tok<<<(unsigned)(want < cap_t ? want : cap_t), CE_WARPS * 32, ce_smem_bytes<CoopTok>(), st>>>(
-      n, in, (const u64*)in_off, ir, list, list_n);
+                                const uint32_t* list, const GgrList* list_h, int sm_count) {
+  k_encode_coop_tok<<<ggr_persistent_grid(n, CE_WARPS, sm_count, CE_TOK_BLOCKS), CE_WARPS * 32, ce_smem_bytes<CoopTok>(), st>>>(
+      n, in, (const u64*)in_off, ir, list, list_h);
 }
 
 void ggr_launch_encode_coop_parse(cudaStream_t st, int tier, long long n, const uint8_t* blob, uint32_t n_msgs,
                                   const int32_t* msg_id, const uint8_t* in, const uint64_t* in_off, uint8_t* ir, uint32_t* size,
                                   uint32_t* first, int32_t* status, uint32_t* ioff, uint32_t* nnodes, const uint32_t* list,
-                                  const uint32_t* list_n, uint32_t* pending, uint32_t* n_pending, int sm_count, int32_t* method,
+                                  const GgrList* list_h, uint32_t* pending, GgrList* pending_h, int sm_count, int32_t* method,
                                   uint32_t* id_span, int32_t final_status) {
   const bool env = method != nullptr;
   if (tier == 0) {
-    // 4 resident blocks per SM (shared memory); never more blocks than items / CE_WARPS
-    long long want = (n + CE_WARPS - 1) / CE_WARPS, cap = (long long)sm_count * 4;
-    unsigned nb = (unsigned)(want < cap ? want : cap);
-    if (env) ce_launch<CoopEnc, true, true>(st, nb, n, blob, n_msgs, msg_id, in, in_off, ir, size, first, status, ioff, nnodes, list, list_n, pending, n_pending, method, id_span, final_status);
-    else ce_launch<CoopEnc, false, true>(st, nb, n, blob, n_msgs, msg_id, in, in_off, ir, size, first, status, ioff, nnodes, list, list_n, pending, n_pending, method, id_span, final_status);
+    // 4 resident blocks per SM (shared memory)
+    const unsigned nb = ggr_persistent_grid(n, CE_WARPS, sm_count, 4);
+    if (env) ce_launch<CoopEnc, true, true>(st, nb, n, blob, n_msgs, msg_id, in, in_off, ir, size, first, status, ioff, nnodes, list, list_h, pending, pending_h, method, id_span, final_status);
+    else ce_launch<CoopEnc, false, true>(st, nb, n, blob, n_msgs, msg_id, in, in_off, ir, size, first, status, ioff, nnodes, list, list_h, pending, pending_h, method, id_span, final_status);
   } else {
     // the list length lives on the device: two blocks per SM (shared memory), warps stride over the list
-    unsigned nb = (unsigned)sm_count * 2u;
-    if (env) ce_launch<CoopEncBig, true, false>(st, nb, n, blob, n_msgs, msg_id, in, in_off, ir, size, first, status, ioff, nnodes, list, list_n, pending, n_pending, method, id_span, final_status);
-    else ce_launch<CoopEncBig, false, false>(st, nb, n, blob, n_msgs, msg_id, in, in_off, ir, size, first, status, ioff, nnodes, list, list_n, pending, n_pending, method, id_span, final_status);
+    const unsigned nb = (unsigned)sm_count * 2u;
+    if (env) ce_launch<CoopEncBig, true, false>(st, nb, n, blob, n_msgs, msg_id, in, in_off, ir, size, first, status, ioff, nnodes, list, list_h, pending, pending_h, method, id_span, final_status);
+    else ce_launch<CoopEncBig, false, false>(st, nb, n, blob, n_msgs, msg_id, in, in_off, ir, size, first, status, ioff, nnodes, list, list_h, pending, pending_h, method, id_span, final_status);
   }
 }
 
 void ggr_launch_encode_coop_emit(cudaStream_t st, long long n, const uint8_t* in, const uint64_t* in_off, const uint8_t* ir,
                                  const uint32_t* ioff, const uint32_t* nnodes, const uint32_t* size, const int32_t* status,
                                  uint8_t* out, const uint64_t* out_off, int sm_count, const uint32_t* list,
-                                 const uint32_t* list_n, uint32_t frame) {
-  static int per_sm = 0;  // resident blocks per SM: what the staging buffers in shared memory (and the registers) allow
-  if (per_sm == 0 && (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_encode_coop_emit, CE_WARPS * 32, sizeof(CoopEmit) * CE_WARPS) != cudaSuccess || per_sm < 1))
-    per_sm = 6;
-  long long want = (n + CE_WARPS - 1) / CE_WARPS, cap = (long long)sm_count * per_sm;
-  unsigned nb = (unsigned)(want < cap ? want : cap);
-  k_encode_coop_emit<<<nb, CE_WARPS * 32, sizeof(CoopEmit) * CE_WARPS, st>>>(n, in, (const u64*)in_off, ir, ioff, nnodes, size, status, out,
-                                                                             (const u64*)out_off, list, list_n, frame);
+                                 const GgrList* list_h, uint32_t frame) {
+  // resident blocks per SM: what the staging buffers in shared memory (and the registers) allow
+  static const int resident = ggr_resident_blocks((const void*)k_encode_coop_emit, CE_WARPS * 32, sizeof(CoopEmit) * CE_WARPS, 6);
+  k_encode_coop_emit<<<ggr_persistent_grid(n, CE_WARPS, sm_count, resident), CE_WARPS * 32, sizeof(CoopEmit) * CE_WARPS, st>>>(
+      n, in, (const u64*)in_off, ir, ioff, nnodes, size, status, out, (const u64*)out_off, list, list_h, frame);
 }

@@ -35,14 +35,14 @@ k_encode_parse(const u8* __restrict__ blob, long long n, u32 n_msgs, const i32* 
   res.first = GGR_NIL;
   {
     Tables T = ggr_tables(blob);
-    // IR region of item i: nodes [(a - a0) / 2 + 8 i, (b - a0) / 2 + 8 (i + 1)), a0 = first offset of the batch
     const u64 a0 = in_off[0];
-    u64 node_off = active ? ((a - a0) >> 1) + 8ull * (u64)i : 0ull;
-    u32 cap = active ? (u32)((((b - a0) >> 1) + 8ull * (u64)(i + 1)) - node_off) : 0u;
+    const GgrRegion r = ggr_item_region(a0, a, b, (u64)i);
+    const u64 node_off = active ? r.node_off : 0ull;
+    const u32 cap = active ? r.cap : 0u;
     const u8* base = in + (a & ~15ull);  // per-item rebasing keeps positions in 32 bits
     u32 s0 = (u32)(a & 15ull);
-    int r = encode_parse(T, (u32)m, base, s0, s0 + (u32)(b - a), ir + node_off * 16, cap, &res, active, GGR_FULL_MASK);
-    if (active) st = r;
+    int rc = encode_parse(T, (u32)m, base, s0, s0 + (u32)(b - a), ir + node_off * 16, cap, &res, active, GGR_FULL_MASK);
+    if (active) st = rc;
   }
   if (i < n) {
     if (st != GST_OK) res.size = 0;
@@ -100,7 +100,7 @@ k_encode_emit(long long n, const u8* __restrict__ in, const u64* __restrict__ in
       }
     }
   }
-  u64 node_off = active ? ((a - in_off[0]) >> 1) + 8ull * (u64)i : 0ull;
+  u64 node_off = active ? ggr_item_region(in_off[0], a, b, (u64)i).node_off : 0ull;
   const u8* base = in + (a & ~15ull);
   u32 s0 = (u32)(a & 15ull);
   if (frame && i < n && sz != 0 && status[i] == GST_OK) {  // message header: every framed item, whoever writes its payload

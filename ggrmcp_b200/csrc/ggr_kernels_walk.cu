@@ -14,7 +14,7 @@
 
 __global__ void __launch_bounds__(CW_WARPS * 32, CW_TOK_BLOCKS)
 k_encode_tok3(const u8* __restrict__ in, const u64* __restrict__ in_off, u8* __restrict__ ir, const u32* __restrict__ list,
-              const u32* __restrict__ list_n) {
+              const GgrList* __restrict__ list_h) {
   __shared__ CwLut lut;
   __shared__ CwTile tiles[CW_WARPS];  // per warp: two 2 KB stages of the item's text, filled by bulk copies (ggr_walk.cuh)
   const u32 warp = threadIdx.x >> 5;
@@ -22,38 +22,36 @@ k_encode_tok3(const u8* __restrict__ in, const u64* __restrict__ in_off, u8* __r
   if ((threadIdx.x & 31u) == 0) cw_tile_init(&tiles[warp]);
   __syncthreads();
   u32 ph = 0;
-  const long long total = (long long)*list_n;
+  const long long total = (long long)list_h->n;
   const u64 a0 = in_off[0];
-  u32* ticket = const_cast<u32*>(list_n) + 1;  // zeroed with the list length
+  u32* ticket = const_cast<u32*>(&list_h->tok_ticket);
   u32 drawn = wp_ticket_draw(ticket);
   for (long long slot = wp_ticket_take(drawn); slot < total; slot = wp_ticket_take(drawn)) {
     drawn = wp_ticket_draw(ticket);
     const long long item = (long long)list[slot];
     const u64 a = in_off[item], b = in_off[item + 1];
     if (b < a || b - a > (u64)CE_MAX_INPUT - 16u) continue;
-    const u64 node_off = ((a - a0) >> 1) + 8ull * (u64)item;
-    const u32 cap = (u32)((((b - a0) >> 1) + 8ull * (u64)(item + 1)) - node_off);
+    const GgrRegion r = ggr_item_region(a0, a, b, (u64)item);
     const u32 s0 = (u32)(a & 15ull);
-    cw_tok_item(&tiles[warp], ph, lut, in + (a & ~15ull), s0, s0 + (u32)(b - a), ir + node_off * 16, cap);
+    cw_tok_item(&tiles[warp], ph, lut, in + (a & ~15ull), s0, s0 + (u32)(b - a), ir + r.node_off * 16, r.cap);
   }
 }
 
 __global__ void __launch_bounds__(CW_WARPS * 32, CW_PLACE_BLOCKS)
-k_encode_place(const u64* __restrict__ in_off, u8* __restrict__ ir, const u32* __restrict__ list, const u32* __restrict__ list_n) {
+k_encode_place(const u64* __restrict__ in_off, u8* __restrict__ ir, const u32* __restrict__ list, const GgrList* __restrict__ list_h) {
   __shared__ CwPlaceSh S[CW_WARPS];
   const u32 warp = threadIdx.x >> 5;
-  const long long total = (long long)*list_n;
+  const long long total = (long long)list_h->n;
   const u64 a0 = in_off[0];
-  u32* ticket = const_cast<u32*>(list_n) + 3;
+  u32* ticket = const_cast<u32*>(&list_h->place_ticket);
   u32 drawn = wp_ticket_draw(ticket);
   for (long long slot = wp_ticket_take(drawn); slot < total; slot = wp_ticket_take(drawn)) {
     drawn = wp_ticket_draw(ticket);
     const long long item = (long long)list[slot];
     const u64 a = in_off[item], b = in_off[item + 1];
     if (b <= a || b - a > (u64)CE_MAX_INPUT - 16u) continue;
-    const u64 node_off = ((a - a0) >> 1) + 8ull * (u64)item;
-    const u32 cap = (u32)((((b - a0) >> 1) + 8ull * (u64)(item + 1)) - node_off);
-    cw_place_item(S[warp], ir + node_off * 16, cap, CoopWalkHuge::MAX_NODE);
+    const GgrRegion r = ggr_item_region(a0, a, b, (u64)item);
+    cw_place_item(S[warp], ir + r.node_off * 16, r.cap, CoopWalkHuge::MAX_NODE);
   }
 }
 
@@ -68,14 +66,14 @@ __global__ void __launch_bounds__(WARPS * 32, FULL ? 1 : CW_WALK_BLOCKS)
 k_encode_type(const u8* __restrict__ blob, u32 n_msgs, const i32* __restrict__ msg_id, const u8* __restrict__ in,
               const u64* __restrict__ in_off, u8* __restrict__ ir, u32* __restrict__ size, u32* __restrict__ first,
               i32* __restrict__ status, u32* __restrict__ ioff, u32* __restrict__ nnodes, const u32* __restrict__ list,
-              const u32* __restrict__ list_n, u32* __restrict__ pending, u32* __restrict__ n_pending) {
+              const GgrList* __restrict__ list_h, u32* __restrict__ pending, GgrList* __restrict__ pending_h) {
   extern __shared__ __align__(16) unsigned char smem[];
   SH* S = reinterpret_cast<SH*>(smem);
   const u32 warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const long long total = (long long)*list_n;
+  const long long total = (long long)list_h->n;
   const Tables T = ggr_tables(blob);
   const u64 a0 = in_off[0];
-  u32* ticket = const_cast<u32*>(list_n) + 2;  // +1 the tokenizer, +3 the place kernel
+  u32* ticket = const_cast<u32*>(&list_h->item_ticket);
   // two tickets in flight (the draw's latency stays off the path).  A bulk L2 prefetch of the next item's index, records
   // and text (cp.async.bulk.prefetch.L2) cost more than it saved here when tuned before the H100 port: the index was written by the two kernels in
   // front of this one and is L2-resident already
@@ -94,10 +92,9 @@ k_encode_type(const u8* __restrict__ blob, u32 n_msgs, const i32* __restrict__ m
     res.n_nodes = 0;
     res.method = 0;
     if (m >= 0 && (u32)m < n_msgs && b >= a && b - a <= (u64)CE_MAX_INPUT - 16u) {
-      const u64 node_off = ((a - a0) >> 1) + 8ull * (u64)item;
-      const u32 cap = (u32)((((b - a0) >> 1) + 8ull * (u64)(item + 1)) - node_off);
+      const GgrRegion r = ggr_item_region(a0, a, b, (u64)item);
       const u32 s0 = (u32)(a & 15ull);
-      ok = cw_type_item<SH, FULL>(S[warp], T, (u32)m, in + (a & ~15ull), s0, s0 + (u32)(b - a), ir + node_off * 16, ioff + node_off, cap, &res);
+      ok = cw_type_item<SH, FULL>(S[warp], T, (u32)m, in + (a & ~15ull), s0, s0 + (u32)(b - a), ir + r.node_off * 16, ioff + r.node_off, r.cap, &res);
     }
     if (lane == 0) {
       if (ok) {
@@ -109,7 +106,7 @@ k_encode_type(const u8* __restrict__ blob, u32 n_msgs, const i32* __restrict__ m
         size[item] = 0;
         nnodes[item] = 0;
         first[item] = GGR_NIL;
-        pending[atomicAdd(n_pending, 1u)] = (u32)item;
+        pending[atomicAdd(&pending_h->n, 1u)] = (u32)item;
       }
     }
     slot = next;
@@ -124,50 +121,37 @@ int ggr_encode_walk_init() {
              : -1;
 }
 
-static unsigned cw_grid(const void* fn, int threads, size_t smem, long long n, int sm_count) {
-  int per_sm = 0;
-  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, threads, smem) != cudaSuccess || per_sm < 1) per_sm = 1;
-  const long long want = (n + CW_WARPS - 1) / CW_WARPS, cap = (long long)sm_count * per_sm;
-  return (unsigned)(want < cap ? (want > 0 ? want : 1) : cap);
-}
-
 void ggr_launch_encode_tok2(cudaStream_t st, long long n, const uint8_t* in, const uint64_t* in_off, uint8_t* ir, const uint32_t* list,
-                            const uint32_t* list_n, int sm_count) {
-  static unsigned per_sm = 0;
-  if (!per_sm) per_sm = cw_grid((const void*)k_encode_tok3, CW_WARPS * 32, 0, 1ll << 40, 1);
-  const long long want = (n + CW_WARPS - 1) / CW_WARPS, cap = (long long)sm_count * per_sm;
-  k_encode_tok3<<<(unsigned)(want < cap ? want : cap), CW_WARPS * 32, 0, st>>>(in, (const u64*)in_off, ir, list, list_n);
+                            const GgrList* list_h, int sm_count) {
+  static const int resident = ggr_resident_blocks((const void*)k_encode_tok3, CW_WARPS * 32, 0, 1);
+  k_encode_tok3<<<ggr_persistent_grid(n, CW_WARPS, sm_count, resident), CW_WARPS * 32, 0, st>>>(in, (const u64*)in_off, ir, list, list_h);
 }
 
-void ggr_launch_encode_place(cudaStream_t st, long long n, const uint64_t* in_off, uint8_t* ir, const uint32_t* list, const uint32_t* list_n,
+void ggr_launch_encode_place(cudaStream_t st, long long n, const uint64_t* in_off, uint8_t* ir, const uint32_t* list, const GgrList* list_h,
                              int sm_count) {
-  static unsigned per_sm = 0;
-  if (!per_sm) per_sm = cw_grid((const void*)k_encode_place, CW_WARPS * 32, 0, 1ll << 40, 1);
-  const long long want = (n + CW_WARPS - 1) / CW_WARPS, cap = (long long)sm_count * per_sm;
-  k_encode_place<<<(unsigned)(want < cap ? want : cap), CW_WARPS * 32, 0, st>>>((const u64*)in_off, ir, list, list_n);
+  static const int resident = ggr_resident_blocks((const void*)k_encode_place, CW_WARPS * 32, 0, 1);
+  k_encode_place<<<ggr_persistent_grid(n, CW_WARPS, sm_count, resident), CW_WARPS * 32, 0, st>>>((const u64*)in_off, ir, list, list_h);
 }
 
-// tier 0: the listed items; tier 1: what tier 0 left (list / list_n = its pending list; the length lives on the device)
+// tier 0: the listed items; tier 1: what tier 0 left (list / list_h = its pending list; the length lives on the device)
 void ggr_launch_encode_type(cudaStream_t st, int tier, long long n, const uint8_t* blob, uint32_t n_msgs, const int32_t* msg_id, const uint8_t* in,
                             const uint64_t* in_off, uint8_t* ir, uint32_t* size, uint32_t* first, int32_t* status, uint32_t* ioff,
-                            uint32_t* nnodes, const uint32_t* list, const uint32_t* list_n, uint32_t* pending, uint32_t* n_pending,
+                            uint32_t* nnodes, const uint32_t* list, const GgrList* list_h, uint32_t* pending, GgrList* pending_h,
                             int sm_count) {
   if (tier == 0) {
-    static unsigned per_sm = 0;
     const size_t smem = sizeof(CoopWalk) * CW_WARPS;
-    if (!per_sm) per_sm = cw_grid((const void*)k_encode_type<CoopWalk, false, CW_WARPS>, CW_WARPS * 32, smem, 1ll << 40, 1);
-    const long long want = (n + CW_WARPS - 1) / CW_WARPS, cap = (long long)sm_count * per_sm;
-    k_encode_type<CoopWalk, false, CW_WARPS><<<(unsigned)(want < cap ? want : cap), CW_WARPS * 32, smem, st>>>(
-        blob, n_msgs, msg_id, in, (const u64*)in_off, ir, size, first, status, ioff, nnodes, list, list_n, pending, n_pending);
+    static const int resident = ggr_resident_blocks((const void*)k_encode_type<CoopWalk, false, CW_WARPS>, CW_WARPS * 32, smem, 1);
+    k_encode_type<CoopWalk, false, CW_WARPS><<<ggr_persistent_grid(n, CW_WARPS, sm_count, resident), CW_WARPS * 32, smem, st>>>(
+        blob, n_msgs, msg_id, in, (const u64*)in_off, ir, size, first, status, ioff, nnodes, list, list_h, pending, pending_h);
   } else if (tier == 2) {
     // third tier: one warp per SM over what the second left
     k_encode_type<CoopWalkHuge, true, 1><<<(unsigned)sm_count, 32, sizeof(CoopWalkHuge), st>>>(
-        blob, n_msgs, msg_id, in, (const u64*)in_off, ir, size, first, status, ioff, nnodes, list, list_n, pending, n_pending);
+        blob, n_msgs, msg_id, in, (const u64*)in_off, ir, size, first, status, ioff, nnodes, list, list_h, pending, pending_h);
   } else {
-    static unsigned per_sm = 0;
+    // the list length lives on the device: every resident block
     const size_t smem = sizeof(CoopWalkBig) * CW_WARPS;
-    if (!per_sm) per_sm = cw_grid((const void*)k_encode_type<CoopWalkBig, true, CW_WARPS>, CW_WARPS * 32, smem, 1ll << 40, 1);
-    k_encode_type<CoopWalkBig, true, CW_WARPS><<<(unsigned)sm_count * per_sm, CW_WARPS * 32, smem, st>>>(
-        blob, n_msgs, msg_id, in, (const u64*)in_off, ir, size, first, status, ioff, nnodes, list, list_n, pending, n_pending);
+    static const int resident = ggr_resident_blocks((const void*)k_encode_type<CoopWalkBig, true, CW_WARPS>, CW_WARPS * 32, smem, 1);
+    k_encode_type<CoopWalkBig, true, CW_WARPS><<<(unsigned)(sm_count * resident), CW_WARPS * 32, smem, st>>>(
+        blob, n_msgs, msg_id, in, (const u64*)in_off, ir, size, first, status, ioff, nnodes, list, list_h, pending, pending_h);
   }
 }

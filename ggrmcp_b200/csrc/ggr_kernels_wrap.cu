@@ -48,13 +48,9 @@ k_wrap_write(long long n, const u8* __restrict__ text, const u64* __restrict__ t
   }
 }
 
-static unsigned wrap_grid(long long n, int sm_count) {
-  long long want = (n + WRAP_WARPS - 1) / WRAP_WARPS, cap = (long long)sm_count * 8;
-  return (unsigned)(want < cap ? want : cap);
-}
 void ggr_launch_wrap_size(cudaStream_t st, long long n, const uint8_t* text, const uint64_t* text_off, const int32_t* status,
                           const uint64_t* ids_off, uint32_t* size, int sm_count) {
-  k_wrap_size<<<wrap_grid(n, sm_count), WRAP_WARPS * 32, 0, st>>>(n, text, (const u64*)text_off, status, (const u64*)ids_off, size);
+  k_wrap_size<<<ggr_persistent_grid(n, WRAP_WARPS, sm_count, 8), WRAP_WARPS * 32, 0, st>>>(n, text, (const u64*)text_off, status, (const u64*)ids_off, size);
 }
 void ggr_launch_offsets(cudaStream_t st, unsigned nb, long long n, const uint32_t* size, const uint64_t* block_prefix,
                         uint64_t* out_off) {
@@ -63,6 +59,6 @@ void ggr_launch_offsets(cudaStream_t st, unsigned nb, long long n, const uint32_
 void ggr_launch_wrap_write(cudaStream_t st, long long n, const uint8_t* text, const uint64_t* text_off, int32_t* status,
                            const uint8_t* ids, const uint64_t* ids_off, const uint32_t* size, uint8_t* out, uint64_t out_cap,
                            const uint64_t* out_off, int sm_count) {
-  k_wrap_write<<<wrap_grid(n, sm_count), WRAP_WARPS * 32, 0, st>>>(n, text, (const u64*)text_off, status, ids, (const u64*)ids_off, size,
+  k_wrap_write<<<ggr_persistent_grid(n, WRAP_WARPS, sm_count, 8), WRAP_WARPS * 32, 0, st>>>(n, text, (const u64*)text_off, status, ids, (const u64*)ids_off, size,
                                                                   out, (u64)out_cap, (const u64*)out_off);
 }

@@ -13,6 +13,7 @@
 #include <stdint.h>
 #include <string.h>
 
+#include "ggr_layout.h"
 #include "ggr_tables.h"
 
 #if defined(__CUDACC__)

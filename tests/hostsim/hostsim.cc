@@ -62,7 +62,7 @@ int hs_encode(void* h, int msg, const uint8_t* json, uint32_t n, uint32_t in_off
   std::vector<uint8_t> inbuf_raw(in_off + n + 64 + 16, 0xEE);
   uint8_t* in = (uint8_t*)(((uintptr_t)inbuf_raw.data() + 15) & ~(uintptr_t)15);
   memcpy(in + in_off, json, n);
-  uint32_t ir_cap = n / 2 + 8;
+  uint32_t ir_cap = ggr_item_region(in_off, in_off, in_off + n, 0).cap;
   uint8_t* ir = (uint8_t*)aligned_alloc(16, (size_t)ir_cap * 16);
   Tables T = ggr_tables(s->blob);
   EncResult res;
@@ -152,7 +152,7 @@ static int hs_encode_coop_t(void* h, int msg, const uint8_t* json, uint32_t n, u
   std::vector<uint8_t> inbuf_raw(in_off + n + 64 + 16, 0xEE);
   uint8_t* in = (uint8_t*)(((uintptr_t)inbuf_raw.data() + 15) & ~(uintptr_t)15);
   memcpy(in + in_off, json, n);
-  uint32_t ir_cap = n / 2 + 8;
+  uint32_t ir_cap = ggr_item_region(in_off, in_off, in_off + n, 0).cap;
   uint8_t* ir = (uint8_t*)aligned_alloc(16, (size_t)ir_cap * 16);
   memset(ir, 0xCC, (size_t)ir_cap * 16);
   static SH S;
@@ -297,7 +297,7 @@ extern "C" int hs_encode_walk(void* h, int msg, const uint8_t* json, uint32_t n,
   std::vector<uint8_t> inbuf_raw(in_off + n + 64 + 16, 0xEE);
   uint8_t* in = (uint8_t*)(((uintptr_t)inbuf_raw.data() + 15) & ~(uintptr_t)15);
   memcpy(in + in_off, json, n);
-  uint32_t cap = n / 2 + 8;  // as the kernels lay the regions out: 8 bytes of IR per input byte + 128
+  uint32_t cap = ggr_item_region(in_off, in_off, in_off + n, 0).cap;  // the region of the batch's first item
   uint8_t* region = (uint8_t*)aligned_alloc(16, (size_t)cap * 16 + 16);
   // what an earlier batch may have left there: well-formed IR nodes (a varint leaf with a two-byte tag), so that a
   // record the walker forgets to write shows up in the output
