@@ -337,6 +337,37 @@ WKT_ENCODE = [(WK, j) for j in [
       ("wkt.HasStruct", b'{"x":1}'), ("wkt.HasStruct", b'{"s":{"a":1}}'), ("wkt.HasStruct", b'{"s":null,"x":2}')]
 
 
+def request_bodies(oracle):
+    """JSON-RPC tools/call request bodies: the reference's pinned bodies, random arguments under varied ids with one
+    damaged or refused variant each, number edge cases, and 400 bench-shaped bodies"""
+    import benchgen
+    from test_oracle import K_BODIES
+    by_input = {m["input"]: (i, m["tool"]) for i, m in reversed(list(enumerate(oracle.methods())))}
+    rng = random.Random(77)
+    bodies = [b[0] for b in K_BODIES]
+    for i, (name, js) in enumerate(random_encode_cases(40, seed0=15000)):
+        k = oracle.msg(name)
+        if k not in by_input:
+            continue
+        tool = by_input[k][1].encode()
+        idt = rng.choice([b"1", b"42", b'"abc"', b"-7", b"123456789012345", b"1.0", b'"a<b"', b"9007199254740993", b"null"])
+        body = b'{"jsonrpc":"2.0","id":' + idt + b',"method":"tools/call","params":{"name":"' + tool + b'","arguments":' + js + b"}}"
+        bodies.append(body)
+        bodies.append([body.replace(b'"2.0"', b'"1.0"'), body.replace(b"tools/call", b"tools/list"), body[:-1] + b',"x":1}',
+                       body.replace(b",", b" ,\n"), body[: len(body) // 2], b""][i % 6])
+    for i, args in enumerate([b'{"f_double":1.5,"f_float":0.1,"f_int32":1e2,"f_uint64":18446744073709551615}', b'{"f_int64":9007199254740993}',
+                              b'{"f_double":1e400}', b'{"f_float":3.4028236e38}', b'{"r_double":[0.30000000000000004,-0.0,4.9e-324]}',
+                              b'{"f_sint64":-1.0,"f_fixed32":4294967295.0}', b'{"f_int32":1.5}']):
+        bodies.append(b'{"jsonrpc":"2.0","id":%d,"method":"tools/call","params":{"name":"bench_benchservice_echoall","arguments":%s}}' % (i, args))
+    wl = benchgen.nested(400, oracle.msg)
+    blob = wl.req_json.tobytes()
+    for i in range(400):
+        js = blob[int(wl.req_off[i]):int(wl.req_off[i + 1])]
+        bodies.append(b'{"jsonrpc":"2.0","id":%d,"method":"tools/call","params":{"name":"%s","arguments":%s}}'
+                      % (i, by_input[int(wl.req_msg[i])][1].encode(), js))
+    return bodies
+
+
 def fieldmask_gap(js):
     """the one documented hole of the FieldMask reader: the JSON string holds escapes"""
     return (b'"fm"' in js or b'"rFm"' in js) and b"\\" in js

@@ -30,8 +30,15 @@ def lib():
         L.hs_request_coop.argtypes = [C.c_void_p, C.c_char_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_char_p, C.c_uint32,
                                       C.POINTER(C.c_uint32), C.POINTER(C.c_uint32), C.c_int]
         L.hs_wrap.argtypes = [C.c_char_p, C.c_uint32, C.c_char_p, C.c_uint32, C.c_char_p, C.c_uint32, C.POINTER(C.c_uint32)]
+        L.hs_keep_state.argtypes = [C.c_int]
         _lib = L
     return _lib
+
+
+def keep_state(on):
+    """on: the lock-step entry points keep their per-warp structures from one item to the next, as persistent warps do;
+    off (the default): every item starts on structures filled with 0xAB"""
+    lib().hs_keep_state(1 if on else 0)
 
 
 def wrap(text, id_tok):

@@ -24,6 +24,15 @@ int g_cw_why = 0;
 extern "C" int hs_cw_why() { return g_cw_why; }
 int g_coop_why = 0;
 extern "C" int hs_coop_why() { return g_coop_why; }
+// A persistent warp keeps its shared memory (and the tables of its kernel) from one item to the next.  By default every
+// lock-step entry point below fills its per-warp structures with 0xAB first, so that a field an item reads before it
+// writes it shows up as garbage.  hs_keep_state(1) skips those fills: item k + 1 then starts with the structures exactly as
+// item k left them, stale state that looks valid, as on the device.
+static int g_keep_state = 0;
+extern "C" void hs_keep_state(int on) { g_keep_state = on; }
+static void item_start_fill(void* p, size_t n, int byte = 0xAB) {
+  if (!g_keep_state) memset(p, byte, n);
+}
 struct HsSchema {
   ggr::CompiledSchema cs;
   uint8_t* blob;  // 16-byte aligned copy
@@ -156,7 +165,7 @@ static int hs_encode_coop_t(void* h, int msg, const uint8_t* json, uint32_t n, u
   uint8_t* ir = (uint8_t*)aligned_alloc(16, (size_t)ir_cap * 16);
   memset(ir, 0xCC, (size_t)ir_cap * 16);
   static SH S;
-  memset(&S, 0xAB, sizeof S);  // stale shared memory must not matter
+  item_start_fill(&S, sizeof S);  // stale shared memory must not matter
   CoopEncArgs<SH> a;
   a.S = &S;
   a.lut = &lut;
@@ -172,7 +181,7 @@ static int hs_encode_coop_t(void* h, int msg, const uint8_t* json, uint32_t n, u
   a.envelope = env_out != nullptr;
   int werr;
   if (SH::MAX_TOK == CoopEnc::MAX_TOK) {
-    memset(&g_tok_state, 0xAB, sizeof g_tok_state);
+    item_start_fill(&g_tok_state, sizeof g_tok_state);
     werr = hw_run_warp(coop_tok_body<SH>, &a);
     if (!werr) werr = hw_run_warp(coop_enc_pre_body<SH>, &a);
   } else {
@@ -219,7 +228,7 @@ static int hs_encode_coop_t(void* h, int msg, const uint8_t* json, uint32_t n, u
     memcpy(ref.data(), rb + out_off, res.size);
   }
   alignas(16) static CoopEmit E;
-  memset(&E, 0xAB, sizeof E);
+  item_start_fill(&E, sizeof E);
   a.E = &E;
   a.dst = ob + out_off;
   if (res.size && res.size <= CE_STAGE) {
@@ -307,9 +316,9 @@ extern "C" int hs_encode_walk(void* h, int msg, const uint8_t* json, uint32_t n,
     memcpy(region + k * 16, stale, 16);
   }
   static CoopWalk S;
-  memset(&S, 0xAB, sizeof S);
+  item_start_fill(&S, sizeof S);
   static CwPlaceSh P;
-  memset(&P, 0xAB, sizeof P);
+  item_start_fill(&P, sizeof P);
   WalkArgs a;
   a.S = &S;
   a.P = &P;
@@ -334,14 +343,14 @@ extern "C" int hs_encode_walk(void* h, int msg, const uint8_t* json, uint32_t n,
   if (!werr) werr = hw_run_warp(walk_place_body, &a);
   if (getenv("HS_DEBUG")) fprintf(stderr, "place: n_rec=%u\n", ((const u32*)region)[3]);
   static CoopWalkBig SB;
-  memset(&SB, 0xAB, sizeof SB);
+  item_start_fill(&SB, sizeof SB);
   a.SB = &SB;
   if (!werr) werr = hw_run_warp(walk_body, &a);
   // what the first tier leaves goes to the second (all leaf forms, 1024 values, items of any size)
   if (!werr && !a.ok[0] && !getenv("HS_WALK_TIER1_ONLY")) werr = hw_run_warp(walk_body_full, &a);
   // ... and what the second leaves (more than 1024 values) to the third
   if (!werr && !a.ok[0] && !getenv("HS_WALK_TIER1_ONLY") && !getenv("HS_WALK_TIER2_ONLY")) {
-    memset(&g_walk_huge, 0xAB, sizeof g_walk_huge);
+    item_start_fill(&g_walk_huge, sizeof g_walk_huge);
     werr = hw_run_warp(walk_body_huge, &a);
   }
   if (werr) {
@@ -371,7 +380,7 @@ extern "C" int hs_encode_walk(void* h, int msg, const uint8_t* json, uint32_t n,
   uint8_t* ob = (uint8_t*)(((uintptr_t)ob_raw.data() + 15) & ~(uintptr_t)15);
   std::vector<uint8_t> before(ob, ob + out_off + res.size + 32);
   alignas(16) static CoopEmit E;
-  memset(&E, 0xAB, sizeof E);
+  item_start_fill(&E, sizeof E);
   a.E = &E;
   a.dst = ob + out_off;
   if (res.size && res.n_nodes > 1) {
@@ -518,7 +527,7 @@ int hs_decode_coop(void* h, int msg, const uint8_t* wire, uint32_t n, uint32_t i
   uint8_t* in = (uint8_t*)(((uintptr_t)inbuf_raw.data() + 15) & ~(uintptr_t)15);
   memcpy(in + in_off, wire, n);
   static CoopShared S;
-  memset(&S, 0xAB, sizeof S);
+  item_start_fill(&S, sizeof S);
   std::vector<U4> tab(2 * GGR_COOP_TAB_ENTRIES);
   CoopDecArgs a;
   a.S = &S;
@@ -538,7 +547,7 @@ int hs_decode_coop(void* h, int msg, const uint8_t* wire, uint32_t n, uint32_t i
     g_coop_pool.assign(2 + 2 * (size_t)GGR_COOP_BIG_ENTRIES + 2 * 7, U4{0xCDCDCDCDu, 0xCDCDCDCDu, 0xCDCDCDCDu, 0xCDCDCDCDu});
     memset(g_coop_pool.data(), 0, 32);
     reinterpret_cast<u32*>(g_coop_pool.data())[0] = 7;  // not at the start of the pool
-    memset(&g_coop_big, 0xAB, sizeof g_coop_big);
+    item_start_fill(&g_coop_big, sizeof g_coop_big);
     werr = hw_run_warp(coop_dec_size_big_body, &a);
     if (werr) return 300 + werr;
     for (int l = 1; l < 32; l++)
@@ -554,12 +563,16 @@ int hs_decode_coop(void* h, int msg, const uint8_t* wire, uint32_t n, uint32_t i
   std::vector<uint8_t> ob_raw(out_off + size + 64, 0xDD);
   uint8_t* ob = (uint8_t*)(((uintptr_t)ob_raw.data() + 15) & ~(uintptr_t)15);
   std::vector<uint8_t> before(ob, ob + out_off + size + 32);
-  memset(&S, 0xCD, sizeof S);  // the write pass may rely on the saved table only
+  // the write pass may rely on the saved table only; the next item's size pass starts from S as this one left it
+  static CoopShared S_kept;
+  S_kept = S;
+  memset(&S, 0xCD, sizeof S);
   alignas(16) static CoopStage E;
-  memset(&E, 0xCD, sizeof E);
+  item_start_fill(&E, sizeof E, 0xCD);
   a.E = &E;
   a.dst = ob + out_off;
   werr = hw_run_warp(coop_dec_write_body, &a);
+  S = S_kept;
   if (werr) return 320 + werr;
   int st = GST_OK;
   for (int l = 0; l < 32; l++)
