@@ -8,6 +8,7 @@ One object per translation unit, compiled in parallel, then linked:
   ggr_kernels_coop_enc.cu lock-step request-side parser (one warp per item)
   ggr_kernels_walk.cu token index + token-parallel walker of the request side (one warp per item)
   ggr_kernels_wrap.cu MCP result bodies around the protojson texts
+  ggr_kernels_diag.cu error detail of failing request items (position, key token, protojson-style text)
   ggr_schema.cc       descriptor-table compiler (host)
 """
 import os
@@ -18,7 +19,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(HERE, "build")
 LIB = os.path.join(HERE, "libggrmcp_b200.so")
-UNITS = ["ggr_engine.cu", "ggr_kernels_enc.cu", "ggr_kernels_dec.cu", "ggr_kernels_coop.cu", "ggr_kernels_coop_enc.cu", "ggr_kernels_walk.cu", "ggr_kernels_wrap.cu", "ggr_schema.cc"]
+UNITS = ["ggr_engine.cu", "ggr_kernels_enc.cu", "ggr_kernels_dec.cu", "ggr_kernels_coop.cu", "ggr_kernels_coop_enc.cu", "ggr_kernels_walk.cu", "ggr_kernels_wrap.cu", "ggr_kernels_diag.cu", "ggr_schema.cc"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC",
          "-I" + os.path.join(os.path.dirname(HERE), "include")]

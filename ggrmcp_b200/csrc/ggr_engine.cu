@@ -7,6 +7,8 @@
 //   reply side   : k_decode_size   (size pass over the wire bytes, block sums)
 //                  k_scan_blocks
 //                  k_decode_write  (block-local scan -> final offsets; write pass)
+//   error detail : k_diag_list, k_encode_parse (list mode), k_diag_locate, k_block_sums, k_scan_blocks, k_offsets, k_diag_write
+//                  (ggr_kernels_diag.cu: the failing items of a request batch, their error positions and texts)
 // Items shard across GPUs by batch index on the caller's side (one engine per device); there is
 // no cross-GPU exchange on this path.
 #include <cuda_runtime.h>
@@ -24,6 +26,7 @@
 #include "../../include/ggrmcp_b200.h"
 #include "ggr_kernels.h"
 #include "ggr_schema.h"
+#include "ggr_status.h"
 #include "ggr_tables.h"
 
 typedef uint8_t u8;
@@ -171,12 +174,13 @@ struct DevBuf {
 };
 
 struct Scratch {
-  DevBuf all[14];
+  DevBuf all[15];
   DevBuf &ir = all[0], &size = all[1], &aux = all[2], &sums = all[3], &pend = all[4], &ioff = all[5], &nn = all[6];
   DevBuf &wtext = all[7], &woff = all[8], &wsize = all[9];  // result wrapping: protojson texts, their offsets, body sizes
   DevBuf& sortpool = all[10];  // reply side: (key, position) records of maps whose entries arrive unsorted
   DevBuf &tabpool = all[11], &taboff = all[12];  // reply side, second lock-step tier: pooled entry tables and where each item's table starts
   DevBuf& spread = all[13];                      // per-thread kernels: the list of large items, one per warp (k_spread)
+  DevBuf& diag = all[14];  // error detail: the re-parse's statuses and error positions, text lengths, lines, columns
   Scratch() = default;
   Scratch(const Scratch&) = delete;
 };
@@ -323,6 +327,10 @@ struct DecodeLists {
 struct BodyLists {
   WorkList lockstep, tier1_left, rest;
 };
+// error detail of request items: the items to diagnose
+struct DiagLists {
+  WorkList failing;
+};
 template <class Set>
 static constexpr int list_count() {
   return sizeof(Set) / sizeof(WorkList);
@@ -359,6 +367,16 @@ static int run_batch(ggr_engine* e, const ggr_schema* s, Scratch& sc, int64_t n,
   const int rc = kernels(nb);
   if (rc != GGR_SUCCESS) return rc;
   return cuda_ok(e, cudaGetLastError(), "kernel launch") ? GGR_SUCCESS : GGR_ERR_CUDA;
+}
+
+// GGR_POISON: after the last kernel of a device-buffer call, in stream order
+static void poison_scratch(ggr_engine* e, Scratch& sc, cudaStream_t st) {
+  if (!e || !e->poison) return;
+  DevBuf* bufs[] = {&sc.ir, &sc.size, &sc.aux, &sc.sums, &sc.pend, &sc.ioff, &sc.nn, &sc.diag};
+  for (DevBuf* b : bufs) {
+    const size_t n16 = b->cap / 16;
+    if (b->p && n16) k_poison<<<(unsigned)((n16 + 255) / 256), 256, 0, st>>>((uint4*)b->p, n16);
+  }
 }
 
 // ---- NUMA placement of the host side (no libnuma in the image: sysfs + sched_setaffinity + first touch) ----
@@ -482,12 +500,7 @@ void ggr_host_free(ggr_engine* e, void* p) {
   cudaFreeHost(p);
 }
 
-const char* ggr_status_string(int32_t st) {
-  static const char* names[] = {"ok", "syntax", "unknown_field", "invalid_value", "range", "invalid_utf8", "duplicate",
-                                "oneof_conflict", "depth", "too_large", "bad_wire", "unsupported", "no_space", "internal"};
-  if (st < 0 || st > 13) return "?";
-  return names[st];
-}
+const char* ggr_status_string(int32_t st) { return ggr_status_name(st); }
 
 int ggr_engine_create(const ggr_config* cfg, ggr_engine** out) {
   if (!out) return GGR_ERR_INVALID_ARGUMENT;
@@ -891,87 +904,42 @@ static int run_dev(ggr_engine* e, const ggr_schema* s, Scratch& sc, bool encode,
     return (encode ? run_encode_kernels : run_decode_kernels)(e, s, sc, n, nb, msg_id, in, in_off, in_bytes, out, out_cap, out_off, status,
                                                               flags, st);
   });
-  if (e && e->poison) {  // after the last kernel of the call, in stream order
-    DevBuf* bufs[] = {&sc.ir, &sc.size, &sc.aux, &sc.sums, &sc.pend, &sc.ioff, &sc.nn};
-    for (DevBuf* b : bufs) {
-      const size_t n16 = b->cap / 16;
-      if (b->p && n16) k_poison<<<(unsigned)((n16 + 255) / 256), 256, 0, st>>>((uint4*)b->p, n16);
-    }
-  }
+  poison_scratch(e, sc, st);
   return rc;
 }
 
-// One failing request item through the per-thread parser again (the kernel that owns the request-side semantics),
-// this time asking where it failed; the text is composed on the host from the status, the position and the input bytes.
-int ggr_encode_diagnose(ggr_engine* e, const ggr_schema* s, int32_t msg_id, const uint8_t* json, uint64_t json_len, uint32_t flags,
-                        int32_t* status, uint32_t* err_pos, uint32_t* err_len, char* text, size_t text_cap) {
-  (void)flags;
-  if (!e || !s || (!json && json_len) || !status) return GGR_ERR_INVALID_ARGUMENT;
-  if (json_len > 0x1FFFF0ull) return GGR_ERR_TOO_LARGE;
-  std::lock_guard<std::mutex> g(e->mu);
-  DeviceGuard dg(e->device);
-  const size_t in_cap = ((size_t)json_len + 15) / 16 * 16 + 64;
-  const size_t ir_bytes = ggr_ir_bytes(json_len, 1);
-  // one allocation: input | offsets | message id | size, first, status, error position | block sums | IR
-  const size_t o_off = in_cap, o_msg = o_off + 16, o_res = o_msg + 16, o_sums = o_res + 16, o_ir = o_sums + 16;
-  uint8_t* d = nullptr;
-  if (!cuda_ok(e, cudaMalloc((void**)&d, o_ir + ir_bytes), "cudaMalloc(diagnose)")) return GGR_ERR_CUDA;
-  std::vector<uint8_t> h(o_ir, 0);
-  if (json_len) memcpy(h.data(), json, (size_t)json_len);
-  const uint64_t offs[2] = {0, json_len};
-  memcpy(h.data() + o_off, offs, 16);
-  memcpy(h.data() + o_msg, &msg_id, 4);
-  cudaStream_t st = e->stream;
-  int rc = GGR_SUCCESS;
-  uint32_t res[4] = {0, 0, 0, 0};
-  if (!cuda_ok(e, cudaMemcpyAsync(d, h.data(), o_ir, cudaMemcpyHostToDevice, st), "H2D(diagnose)")) rc = GGR_ERR_CUDA;
-  if (rc == GGR_SUCCESS) {
-    ggr_launch_encode_parse(st, 1, s->d_blob, 1, (u32)s->cs.msg_names.size(), (const int32_t*)(d + o_msg), d, (const uint64_t*)(d + o_off), d + o_ir,
-                            (u32*)(d + o_res), (u32*)(d + o_res + 4), (int32_t*)(d + o_res + 8), (uint64_t*)(d + o_sums), nullptr, nullptr,
-                            (u32*)(d + o_res + 12));
-    e->launches += 1;
-    if (!cuda_ok(e, cudaGetLastError(), "kernel launch") ||
-        !cuda_ok(e, cudaMemcpyAsync(res, d + o_res, 16, cudaMemcpyDeviceToHost, st), "D2H(diagnose)") ||
-        !cuda_ok(e, cudaStreamSynchronize(st), "sync(diagnose)"))
-      rc = GGR_ERR_CUDA;
-  }
-  cudaFree(d);
-  if (rc != GGR_SUCCESS) return rc;
-  const int32_t stt = (int32_t)res[2];
-  *status = stt;
-  uint32_t pos = stt != GGR_ST_OK ? res[3] : 0, len = 0;
-  if (pos > json_len) pos = (uint32_t)json_len;
-  // a key token at the position: its raw text (quotes included) is what protojson prints
-  if (stt != GGR_ST_OK && pos < json_len && json[pos] == '"') {
-    uint64_t q = pos + 1;
-    while (q < json_len && json[q] != '"') q += json[q] == '\\' ? 2 : 1;
-    if (q < json_len) len = (uint32_t)(q + 1 - pos);
-  }
-  if (err_pos) *err_pos = pos;
-  if (err_len) *err_len = len;
-  if (text && text_cap) {
-    std::string t;
-    if (stt == GGR_ST_OK) {
-      t = "";
-    } else {
-      // position as protojson reports it: line and column (in bytes), both from 1
-      uint32_t line = 1, col = 1;
-      for (uint32_t k = 0; k < pos; k++) {
-        if (json[k] == '\n') { line++; col = 1; }
-        else col++;
-      }
-      t = "proto: (line " + std::to_string(line) + ":" + std::to_string(col) + "): ";
-      const std::string tok = len ? std::string((const char*)json + pos, len) : std::string();
-      if (stt == GGR_ST_UNKNOWN_FIELD && len) t += "unknown field " + tok;
-      else if (stt == GGR_ST_DUPLICATE && len) t += "duplicate field " + tok;
-      else if (stt == GGR_ST_ONEOF && len) t += "error parsing " + tok + ", oneof is already set";
-      else t += ggr_status_string(stt);
-    }
-    const size_t k = t.size() < text_cap - 1 ? t.size() : text_cap - 1;
-    memcpy(text, t.data(), k);
-    text[k] = 0;
-  }
-  return GGR_SUCCESS;
+// Error detail of request items (ggr_encode_diagnose_batch[_dev], ggr_encode_diagnose): the list of the items to diagnose
+// (status null: every item), the per-thread parser over them once more in list mode - the kernel that decides every
+// request-side status - with its error positions, in the batch's own IR regions (so this is request-side scratch), then
+// one warp per item for position, key token and text length, the scan of the lengths into text_off, and the texts.
+// Seven launches, however many items fail.  parse_status: where the re-parse's statuses go (null: scratch).
+static int run_diag_dev(ggr_engine* e, const ggr_schema* s, Scratch& sc, int64_t n, const int32_t* msg_id, const uint8_t* in,
+                        const uint64_t* in_off, uint64_t in_bytes, const int32_t* status, uint32_t* err_pos, uint32_t* err_len, uint8_t* text,
+                        uint64_t text_cap, uint64_t* text_off, int32_t* parse_status, cudaStream_t st) {
+  const bool have_args = msg_id && in && in_off && err_pos && err_len && (text || !text_cap);
+  const int rc = run_batch(e, s, sc, n, have_args, in, nullptr, text_off, st, [&](long long nb) {
+    DiagLists L;
+    if (!ensure(e, sc.ir, ggr_ir_bytes(in_bytes, n)) || !ensure(e, sc.diag, (size_t)n * 20) || !make_lists(e, sc.pend, n, st, &L))
+      return GGR_ERR_CUDA;
+    u32* d = (u32*)sc.diag.p;
+    u32 *parse_pos = d + n, *text_len = d + 2 * n, *line = d + 3 * n, *col = d + 4 * n;
+    if (!parse_status) parse_status = (i32*)d;
+    u64* sums = (u64*)sc.sums.p;
+    ggr_launch_diag_list(st, n, status, L.failing.item, L.failing.h, err_pos, err_len, text_len);
+    ggr_launch_encode_parse(st, (unsigned)nb, s->d_blob, n, (u32)s->cs.msg_names.size(), msg_id, in, in_off, (u8*)sc.ir.p, (u32*)sc.size.p,
+                            (u32*)sc.aux.p, parse_status, sums, L.failing.item, &L.failing.h->n, parse_pos);
+    ggr_launch_diag_locate(st, n, in, in_off, parse_status, parse_pos, L.failing.item, L.failing.h, err_pos, err_len, text_len, line, col,
+                           e->sm_count);
+    ggr_launch_block_sums(st, (unsigned)nb, n, text_len, sums);
+    k_scan_blocks<<<1, 1024, 0, st>>>(sums, nb, text_off + n);
+    ggr_launch_offsets(st, (unsigned)nb, n, text_len, sums, text_off);
+    ggr_launch_diag_write(st, n, in, in_off, parse_status, L.failing.item, L.failing.h, err_pos, err_len, text_len, line, col, text, text_cap,
+                          text_off, e->sm_count);
+    e->launches += 7;
+    return GGR_SUCCESS;
+  });
+  poison_scratch(e, sc, st);
+  return rc;
 }
 
 int ggr_encode_batch_dev(ggr_engine* e, const ggr_schema* s, int64_t n, const int32_t* msg_id, const uint8_t* in,
@@ -1382,6 +1350,131 @@ int ggr_request_batch(ggr_engine* e, const ggr_schema* s, int64_t n, const uint8
   if (total && (!cuda_ok(e, cudaMemcpyAsync(out, sl.d_out.p, total, cudaMemcpyDeviceToHost, st), "D2H payload") ||
                 !cuda_ok(e, cudaStreamSynchronize(st), "sync")))
     return GGR_ERR_CUDA;
+  return GGR_SUCCESS;
+}
+
+int ggr_encode_diagnose_batch_dev(ggr_engine* e, const ggr_schema* s, int64_t n, const int32_t* msg_id, const uint8_t* in,
+                                  const uint64_t* in_off, uint64_t in_bytes, const int32_t* status, uint32_t* err_pos, uint32_t* err_len,
+                                  uint8_t* text, uint64_t text_cap, uint64_t* text_off, void* stream) {
+  if (!e || !text_off || (n > 0 && !status)) return GGR_ERR_INVALID_ARGUMENT;
+  std::lock_guard<std::mutex> g(e->mu);
+  return run_diag_dev(e, s, e->dev_sc[0], n, msg_id, in, in_off, in_bytes, status, err_pos, err_len, text, text_cap, text_off, nullptr,
+                      stream ? (cudaStream_t)stream : e->stream);
+}
+
+// Host buffers: k items in[in_off[j] .. in_off[j + 1]) (offsets from 0) of messages msg[j], every one diagnosed, on the
+// request side's first slot (its staging buffers and scratch, as ggr_request_batch uses them).  Returns per item the
+// re-parse's status (when parse_status is given), error position, key token length and text offsets (k + 1 entries), and
+// the packed texts when they fit text_cap (GGR_ERR_NO_SPACE otherwise).  The caller holds mu_host[0] and mu.
+static int diag_host(ggr_engine* e, const ggr_schema* s, int64_t k, const int32_t* msg, const uint8_t* in, const uint64_t* in_off,
+                     int32_t* parse_status, uint32_t* err_pos, uint32_t* err_len, uint64_t* text_off, uint8_t* text, uint64_t text_cap) {
+  DeviceGuard dg(e->device);
+  Slot& sl = e->slots[0][0];
+  if (!slot_init(e, sl)) return GGR_ERR_CUDA;
+  const uint64_t in_bytes = in_off[k];
+  // no text is longer than its item plus 80 bytes, so the device never needs more room than that
+  const uint64_t bound = in_bytes + 80ull * (uint64_t)k, dev_cap = text_cap < bound ? text_cap : bound;
+  if (!ensure(e, sl.d_in, (size_t)in_bytes + 128) || !ensure(e, sl.d_off, (size_t)(k + 1) * 8) || !ensure(e, sl.d_msg, (size_t)k * 4) ||
+      !ensure(e, sl.d_out, (size_t)dev_cap + 64) || !ensure(e, sl.d_out_off, (size_t)(k + 1) * 8) || !ensure(e, sl.d_status, (size_t)k * 4) ||
+      !ensure(e, sl.d_ids_off, (size_t)k * 8))
+    return GGR_ERR_CUDA;
+  cudaStream_t st = sl.st;
+  u8* d_in = (u8*)sl.d_in.p;
+  u32* d_pos = (u32*)sl.d_ids_off.p;  // error positions, then key token lengths
+  if ((in_bytes && !cuda_ok(e, cudaMemcpyAsync(d_in, in, in_bytes, cudaMemcpyHostToDevice, st), "H2D payload")) ||
+      !cuda_ok(e, cudaMemsetAsync(d_in + in_bytes, 0, 64, st), "pad") ||
+      !cuda_ok(e, cudaMemcpyAsync(sl.d_off.p, in_off, (size_t)(k + 1) * 8, cudaMemcpyHostToDevice, st), "H2D offsets") ||
+      !cuda_ok(e, cudaMemcpyAsync(sl.d_msg.p, msg, (size_t)k * 4, cudaMemcpyHostToDevice, st), "H2D ids"))
+    return GGR_ERR_CUDA;
+  const int rc = run_diag_dev(e, s, sl.sc, k, (const int32_t*)sl.d_msg.p, d_in, (const uint64_t*)sl.d_off.p, in_bytes, nullptr, d_pos, d_pos + k,
+                              (uint8_t*)sl.d_out.p, dev_cap, (uint64_t*)sl.d_out_off.p, (int32_t*)sl.d_status.p, st);
+  if (rc != GGR_SUCCESS) return rc;
+  if (!cuda_ok(e, cudaMemcpyAsync(text_off, sl.d_out_off.p, (size_t)(k + 1) * 8, cudaMemcpyDeviceToHost, st), "D2H offsets") ||
+      !cuda_ok(e, cudaMemcpyAsync(err_pos, d_pos, (size_t)k * 4, cudaMemcpyDeviceToHost, st), "D2H positions") ||
+      !cuda_ok(e, cudaMemcpyAsync(err_len, d_pos + k, (size_t)k * 4, cudaMemcpyDeviceToHost, st), "D2H token lengths") ||
+      (parse_status && !cuda_ok(e, cudaMemcpyAsync(parse_status, sl.d_status.p, (size_t)k * 4, cudaMemcpyDeviceToHost, st), "D2H status")) ||
+      !cuda_ok(e, cudaStreamSynchronize(st), "sync"))
+    return GGR_ERR_CUDA;
+  const uint64_t total = text_off[k];
+  if (total > text_cap) return GGR_ERR_NO_SPACE;
+  if (total && (!cuda_ok(e, cudaMemcpyAsync(text, sl.d_out.p, total, cudaMemcpyDeviceToHost, st), "D2H texts") ||
+                !cuda_ok(e, cudaStreamSynchronize(st), "sync")))
+    return GGR_ERR_CUDA;
+  return GGR_SUCCESS;
+}
+
+// Host buffers: only the items to diagnose travel, gathered back to back; their results are put back in the batch's order.
+int ggr_encode_diagnose_batch(ggr_engine* e, const ggr_schema* s, int64_t n, const int32_t* msg_id, const uint8_t* json,
+                              const uint64_t* json_off, const int32_t* status, uint32_t* err_pos, uint32_t* err_len, uint8_t* text,
+                              uint64_t text_cap, uint64_t* text_off) {
+  if (!e || !s || n < 0 || !text_off) return GGR_ERR_INVALID_ARGUMENT;
+  if (n == 0) {
+    text_off[0] = 0;
+    return GGR_SUCCESS;
+  }
+  if (!msg_id || !json || !json_off || !status || !err_pos || !err_len || (!text && text_cap)) return GGR_ERR_INVALID_ARGUMENT;
+  std::vector<int64_t> idx;
+  std::vector<int32_t> msg;
+  std::vector<uint64_t> off(1, 0);
+  for (int64_t i = 0; i < n; i++) {
+    if (status[i] == GGR_ST_OK || status[i] == GGR_ST_NO_SPACE) continue;
+    idx.push_back(i);
+    msg.push_back(msg_id[i]);
+    off.push_back(off.back() + (json_off[i + 1] - json_off[i]));
+  }
+  const int64_t k = (int64_t)idx.size();
+  std::vector<uint8_t> in((size_t)off.back());
+  for (int64_t j = 0; j < k; j++) memcpy(in.data() + off[j], json + json_off[idx[j]], (size_t)(off[j + 1] - off[j]));
+  std::vector<uint32_t> pos((size_t)k), len((size_t)k);
+  std::vector<uint64_t> toff((size_t)k + 1, 0);
+  int rc = GGR_SUCCESS;
+  if (k) {
+    std::lock_guard<std::mutex> g(e->mu_host[0]);
+    std::lock_guard<std::mutex> g2(e->mu);
+    rc = diag_host(e, s, k, msg.data(), in.data(), off.data(), nullptr, pos.data(), len.data(), toff.data(), text, text_cap);
+    if (rc != GGR_SUCCESS && rc != GGR_ERR_NO_SPACE) return rc;
+  }
+  // the items that were not diagnosed have no text, so the packed texts are the batch's already
+  uint64_t at = 0;
+  int64_t j = 0;
+  for (int64_t i = 0; i < n; i++) {
+    text_off[i] = at;
+    const bool listed = j < k && idx[j] == i;
+    err_pos[i] = listed ? pos[j] : 0;
+    err_len[i] = listed ? len[j] : 0;
+    if (listed) {
+      at += toff[j + 1] - toff[j];
+      j++;
+    }
+  }
+  text_off[n] = at;  // GGR_ERR_NO_SPACE: the capacity that would do
+  return rc;
+}
+
+// One item: the batch path with a batch of one, its text cut to text_cap - 1 bytes and NUL-terminated.
+int ggr_encode_diagnose(ggr_engine* e, const ggr_schema* s, int32_t msg_id, const uint8_t* json, uint64_t json_len, uint32_t flags,
+                        int32_t* status, uint32_t* err_pos, uint32_t* err_len, char* text, size_t text_cap) {
+  (void)flags;
+  if (!e || !s || (!json && json_len) || !status) return GGR_ERR_INVALID_ARGUMENT;
+  if (json_len > 0x1FFFF0ull) return GGR_ERR_TOO_LARGE;
+  const uint64_t off[2] = {0, json_len};
+  std::vector<uint8_t> t((size_t)json_len + 80);
+  uint32_t pos = 0, len = 0;
+  uint64_t toff[2] = {0, 0};
+  int rc;
+  {
+    std::lock_guard<std::mutex> g(e->mu_host[0]);
+    std::lock_guard<std::mutex> g2(e->mu);
+    rc = diag_host(e, s, 1, &msg_id, json, off, status, &pos, &len, toff, t.data(), t.size());
+  }
+  if (rc != GGR_SUCCESS) return rc;
+  if (err_pos) *err_pos = pos;
+  if (err_len) *err_len = len;
+  if (text && text_cap) {
+    const size_t k = toff[1] < text_cap - 1 ? (size_t)toff[1] : text_cap - 1;
+    memcpy(text, t.data(), k);
+    text[k] = 0;
+  }
   return GGR_SUCCESS;
 }
 

@@ -81,5 +81,16 @@ void ggr_launch_offsets(cudaStream_t st, unsigned nb, long long n, const uint32_
 void ggr_launch_wrap_write(cudaStream_t st, long long n, const uint8_t* text, const uint64_t* text_off, int32_t* status,
                            const uint8_t* ids, const uint64_t* ids_off, const uint32_t* size, uint8_t* out, uint64_t out_cap,
                            const uint64_t* out_off, int sm_count);
+// error detail of failing request items (ggr_kernels_diag.cu): the list of items to diagnose (status null: every item),
+// then - behind the re-parse - error position, key token, line, column and text length, then the texts
+void ggr_launch_diag_list(cudaStream_t st, long long n, const int32_t* status, uint32_t* list, GgrList* list_h, uint32_t* err_pos,
+                          uint32_t* err_len, uint32_t* text_len);
+void ggr_launch_diag_locate(cudaStream_t st, long long n, const uint8_t* in, const uint64_t* in_off, const int32_t* parse_status,
+                            const uint32_t* parse_pos, const uint32_t* list, const GgrList* list_h, uint32_t* err_pos, uint32_t* err_len,
+                            uint32_t* text_len, uint32_t* line, uint32_t* col, int sm_count);
+void ggr_launch_diag_write(cudaStream_t st, long long n, const uint8_t* in, const uint64_t* in_off, const int32_t* parse_status,
+                           const uint32_t* list, const GgrList* list_h, const uint32_t* err_pos, const uint32_t* err_len,
+                           const uint32_t* text_len, const uint32_t* line, const uint32_t* col, uint8_t* text, uint64_t text_cap,
+                           const uint64_t* text_off, int sm_count);
 const void* ggr_kernel_encode_parse();  // for cudaFuncGetAttributes (is the sm_90a image loadable?)
 int ggr_decode_max_rec();

@@ -77,6 +77,8 @@ def _load():
     L.ggr_request_batch_dev.argtypes = [vp, vp, C.c_int64, vp, vp, C.c_uint64, vp, C.c_uint64, vp, vp, vp, vp, vp]
     L.ggr_decode_wrap_batch.argtypes = [vp, vp, C.c_int64, vp, vp, vp, vp, vp, vp, C.c_uint64, vp, vp, C.c_uint32]
     L.ggr_decode_wrap_batch_dev.argtypes = [vp, vp, C.c_int64, vp, vp, vp, C.c_uint64, vp, vp, vp, C.c_uint64, vp, vp, C.c_uint32, vp]
+    L.ggr_encode_diagnose_batch.argtypes = [vp, vp, C.c_int64, vp, vp, vp, vp, vp, vp, vp, C.c_uint64, vp]
+    L.ggr_encode_diagnose_batch_dev.argtypes = [vp, vp, C.c_int64, vp, vp, vp, C.c_uint64, vp, vp, vp, vp, C.c_uint64, vp, vp]
     L.ggr_synchronize.argtypes = [vp]
     L.ggr_profile_enable.argtypes = [vp, C.c_int]
     L.ggr_profile_read.argtypes = [vp, C.POINTER(C.c_double), C.POINTER(C.c_uint64)]
@@ -224,6 +226,38 @@ class Engine:
         if rc != 0:
             self._err(rc, "ggr_encode_diagnose")
         return st.value, pos.value, ln.value, buf.value.decode("utf-8", "replace")
+
+    def encode_diagnose_batch(self, schema, msg_ids, data, off, status, text_cap=None):
+        """Error detail of every failing item of a request batch (ggr_encode_diagnose_batch), given the batch as
+        encode_batch took it and the statuses it returned: (err_pos[n], err_len[n], texts), texts a list of n bytes
+        objects; items with status 0 (ok) or 12 (no_space) get 0, 0, b""."""
+        n = len(msg_ids)
+        msg_ids = np.ascontiguousarray(msg_ids, dtype=np.int32)
+        off = np.ascontiguousarray(off, dtype=np.uint64)
+        data = np.ascontiguousarray(data, dtype=np.uint8)
+        status = np.ascontiguousarray(status, dtype=np.int32)
+        assert len(off) == n + 1 and len(status) == n
+        if text_cap is None:
+            text_cap = 128 * int(np.count_nonzero((status != 0) & (status != 12))) + 64
+        text = np.empty(max(int(text_cap), 1), dtype=np.uint8)
+        text_off = np.zeros(n + 1, dtype=np.uint64)
+        err_pos = np.zeros(max(n, 1), dtype=np.uint32)
+        err_len = np.zeros(max(n, 1), dtype=np.uint32)
+        rc = _load().ggr_encode_diagnose_batch(self.h, schema.h, n, msg_ids.ctypes.data, data.ctypes.data if len(data) else text.ctypes.data,
+                                               off.ctypes.data, status.ctypes.data, err_pos.ctypes.data, err_len.ctypes.data,
+                                               text.ctypes.data, int(text_cap), text_off.ctypes.data)
+        if rc == -5:
+            return self.encode_diagnose_batch(schema, msg_ids, data, off, status, int(text_off[n]))
+        if rc != 0:
+            self._err(rc, "ggr_encode_diagnose_batch")
+        return err_pos[:n], err_len[:n], unpack(text[: int(text_off[n])], text_off)
+
+    def encode_diagnose_batch_dev(self, schema, n, msg_ids_ptr, in_ptr, in_off_ptr, in_bytes, status_ptr, err_pos_ptr, err_len_ptr,
+                                  text_ptr, text_cap, text_off_ptr, stream=None):
+        rc = _load().ggr_encode_diagnose_batch_dev(self.h, schema.h, n, msg_ids_ptr, in_ptr, in_off_ptr, in_bytes, status_ptr,
+                                                   err_pos_ptr, err_len_ptr, text_ptr, text_cap, text_off_ptr, stream)
+        if rc != 0:
+            self._err(rc, "ggr_encode_diagnose_batch_dev")
 
     def request_batch(self, schema, bodies, off, out_cap=None):
         """JSON-RPC tools/call request bodies -> (wire bytes, offsets[n+1], method[n], id_span[n, 2], status[n]);

@@ -156,7 +156,7 @@ int ggr_decode_batch(ggr_engine* e, const ggr_schema* s, int64_t n, const int32_
  * Same operations on buffers already resident in HBM (all pointers are device pointers on the
  * engine's device; `in` must be 16-byte aligned and readable 64 bytes past its end).  Work is
  * enqueued on `stream` (a cudaStream_t, NULL = the engine's own stream) and not synchronized.
- * The calls of one direction (ggr_encode_batch_dev and ggr_request_batch_dev; ggr_decode_batch_dev and
+ * The calls of one direction (ggr_encode_batch_dev, ggr_request_batch_dev and ggr_encode_diagnose_batch_dev; ggr_decode_batch_dev and
  * ggr_decode_wrap_batch_dev) work in the engine's one scratch area of that direction: two of them on DIFFERENT streams
  * must be ordered by the caller (an event recorded behind the first, waited for by the second stream) - on the same
  * stream they are ordered already; a request-side call and a reply-side call may overlap freely.  The host-buffer
@@ -171,15 +171,41 @@ int ggr_decode_batch_dev(ggr_engine* e, const ggr_schema* s, int64_t n, const in
 int ggr_synchronize(ggr_engine* e);
 
 /*
- * Error detail of ONE request item the batch calls reported with status != 0 (SURVEY.md 8b "Error conventions": the Go
- * side returns `failed to parse input JSON: <protojson's error>`, reflection.go:356, and the reference's tests pin the
- * substring `unknown field` with the offending name, tests/real_grpc_invocation_test.go:238-245).  The item goes through
- * the device's per-thread parser once more (the kernel that decides every request-side error), which reports where it
- * stopped: *err_pos is the byte offset inside json - of the member's key token for unknown fields, duplicate fields and
- * oneof conflicts, of the reader otherwise - and *err_len the length of the key token there (quotes included; 0 when the
- * position is no key).  text (optional, NUL-terminated, truncated to text_cap): `proto: (line L:C): unknown field "x"` /
- * `duplicate field "x"` in protojson's wording, the status name behind the position for the other categories.
- * Synchronous, rare-path (one small allocation per call); *status repeats the batch call's status of the item.
+ * Error detail of the failing items of a request batch (SURVEY.md 8b "Error conventions": the Go side returns
+ * `failed to parse input JSON: <protojson's error>`, reflection.go:356, and the reference's tests pin the substring
+ * `unknown field` with the offending name, tests/real_grpc_invocation_test.go:238-245).  The call takes the batch exactly
+ * as ggr_encode_batch[_dev] took it, and status[] as that call returned it.  Items with status GGR_ST_OK or
+ * GGR_ST_NO_SPACE are not looked at: err_pos[i] = err_len[i] = 0 and an empty text.  Every other item goes through the
+ * device's per-thread parser once more (the kernel that decides every request-side status), which reports where it
+ * stopped:
+ *   err_pos[i]  byte offset inside the item - of the member's key token for unknown fields, duplicate fields and oneof
+ *               conflicts, of the reader otherwise - clamped to the item's length
+ *   err_len[i]  length of the key token there: from the '"' at err_pos to the next '"' no backslash escapes, quotes
+ *               included; 0 when the position holds no key or the token has no closing quote
+ *   text        `proto: (line L:C): unknown field "x"` / `duplicate field "x"` / `error parsing "x", oneof is already set`
+ *               in protojson's wording when a key token was found, the status name (ggr_status_string) behind the
+ *               position otherwise; line and column counted in bytes from 1
+ * Texts are packed without NUL: item i's is text[text_off[i] .. text_off[i+1]) (text_off has n + 1 entries).  When
+ * text_cap is too small the host form returns GGR_ERR_NO_SPACE and text_off[n] holds the capacity that would do; the _dev
+ * form writes only the texts that fit and leaves the same total in text_off[n] for the caller to check.
+ * The kernels launched per call are the same however many items fail.  The host form copies only the items it
+ * diagnoses to the device and works in the request side's host-call scratch (one host-buffer request-side call at a
+ * time, as ggr_encode_batch).  The _dev form takes device pointers laid out as for ggr_encode_batch_dev and enqueues on
+ * `stream`: it is a request-side call - it re-parses into the request side's scratch - so the ordering rule of the
+ * device-buffer calls above holds for it too (behind a ggr_encode_batch_dev of the same batch on the same stream it is
+ * ordered already; on another stream an event must order the two).
+ */
+int ggr_encode_diagnose_batch(ggr_engine* e, const ggr_schema* s, int64_t n, const int32_t* msg_id, const uint8_t* json,
+                              const uint64_t* json_off, const int32_t* status, uint32_t* err_pos, uint32_t* err_len,
+                              uint8_t* text, uint64_t text_cap, uint64_t* text_off);
+int ggr_encode_diagnose_batch_dev(ggr_engine* e, const ggr_schema* s, int64_t n, const int32_t* msg_id, const uint8_t* in,
+                                  const uint64_t* in_off, uint64_t in_bytes, const int32_t* status, uint32_t* err_pos,
+                                  uint32_t* err_len, uint8_t* text, uint64_t text_cap, uint64_t* text_off, void* stream);
+/*
+ * Error detail of ONE request item, whatever its status: ggr_encode_diagnose_batch over a batch of that item alone.
+ * *status is the re-parse's status (the batch call's status of the item); *err_pos, *err_len and text as above, text
+ * (optional) NUL-terminated and truncated to text_cap.  Synchronous; an item above 2 MiB - 16 bytes gives
+ * GGR_ERR_TOO_LARGE.
  */
 int ggr_encode_diagnose(ggr_engine* e, const ggr_schema* s, int32_t msg_id, const uint8_t* json, uint64_t json_len,
                         uint32_t flags, int32_t* status, uint32_t* err_pos, uint32_t* err_len, char* text, size_t text_cap);
