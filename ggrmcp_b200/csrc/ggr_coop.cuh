@@ -9,7 +9,7 @@
 //                 step) so that a string needs no per-byte scan unless it holds a quote, a
 //                 backslash, a control or a non-ASCII byte; entries are bucketed by kind
 //   R3 sizes    : one lane per leaf computes the size of its JSON text; message entries add up
-//                 bottom-up by depth; offsets go top-down
+//                 bottom-up, one level of R1's queue at a time; offsets go top-down
 //   -- the entry table is saved, the batch-wide scan of the item sizes runs --
 //   R4 write    : one lane per entry writes its text at its offset; long plain strings are copied
 //                 by the whole warp
@@ -72,14 +72,14 @@ template <int NE>
 struct CoopSharedT {
   static const u32 ENTRIES = NE;
   CoopEnt ent[NE];
-  union {
-    u16 order[NE];                        // R3: leaves bucketed by class
-    u16 queue[NE];                        // R1: message entries to scan, level by level (done before `order` is filled)
-  };
+  // message entries level by level in [0, q_end) (R1 appends them; R3 closes and places them by level), then the
+  // leaves bucketed by class in [q_end, leaf_end)
+  u16 queue[NE];
+  u16 lvl[GGR_COOP_DEPTH + 1];            // queue index where each level starts (and where the last one ends)
   u16 dmask[GGR_COOP_MAX_WIRE / 16 + 2];  // per 16-byte chunk: bytes that are not plain text
   u16 dpre[GGR_COOP_MAX_WIRE / 16 + 2];   // number of chunks with a nonzero mask before this one
   u32 cls_cnt[DC_N], cls_cur[DC_N];
-  u32 n_ent, bail, n_leaf, max_depth, q_end, n_dirty;
+  u32 n_ent, bail, leaf_end, q_end, n_dirty;
   u16 dlist[GGR_COOP_DIRTY_MAX];          // strings that need escaping / validation: sized by the whole warp
 };
 typedef CoopSharedT<GGR_COOP_ENTRIES> CoopShared;      // first tier
@@ -295,7 +295,6 @@ GGR_DEV void coop_scan_message(SH& S, const DecCtx& cx, u32 me) {
     any = true;
   }
   if (open && prev != 0xFFFFu) S.ent[prev].flags |= CF_ARR_LAST;
-  wp_atomic_max(&S.max_depth, (u32)m.depth + 1u);
 }
 
 // flags in bit 7 of every byte -> 4 contiguous bits
@@ -703,7 +702,6 @@ GGR_DEV bool coop_size_item(SH& S, const DecCtx& cx, u32 root_msg, u32 start, u3
   if (lane == 0) {
     S.n_ent = 1;
     S.bail = 0;
-    S.max_depth = 0;
     S.n_dirty = 0;
     CoopEnt r0;
     r0.vpos = start; r0.vend = end; r0.gfield = GGR_COOP_ROOT; r0.parent = 0xFFFFu; r0.next = 0xFFFFu;
@@ -718,11 +716,13 @@ GGR_DEV bool coop_size_item(SH& S, const DecCtx& cx, u32 root_msg, u32 start, u3
   // R2 first: the plain-text masks read the whole item with coalesced 16-byte loads, which also brings
   // its lines into L1 for the byte-wise discovery below
   if (have_masks) coop_plain_masks(S, cx.in, start, end);
-  // R1: level by level
-  u32 qb = 0;
+  // R1: level by level (level d holds the messages of depth d)
+  u32 qb = 0, nl = 0;
   for (;;) {
     const u32 qe = S.q_end;
+    if (lane == 0) S.lvl[nl] = (u16)qb;
     if (qb == qe) break;
+    nl++;
     WP_SYNC();
     for (u32 i = qb + lane; i < qe; i += 32) coop_scan_message(S, cx, S.queue[i]);
     WP_SYNC();
@@ -738,23 +738,25 @@ GGR_DEV bool coop_size_item(SH& S, const DecCtx& cx, u32 root_msg, u32 start, u3
     if (c != DC_MSG) wp_atomic_add(&S.cls_cnt[c], 1u);
   }
   WP_SYNC();
+  const u32 q_end = S.q_end;
   if (lane == 0) {
-    u32 run = 0;
+    u32 run = q_end;
     for (u32 c = 0; c < DC_N; c++) {
       S.cls_cur[c] = run;
       run += S.cls_cnt[c];
     }
-    S.n_leaf = run;
+    S.leaf_end = run;
   }
   WP_SYNC();
   for (u32 i = lane; i < n; i += 32) {
     const u32 c = CE_CLASS(S.ent[i]);
-    if (c != DC_MSG) S.order[wp_atomic_add(&S.cls_cur[c], 1u)] = (u16)i;
+    if (c != DC_MSG) S.queue[wp_atomic_add(&S.cls_cur[c], 1u)] = (u16)i;
   }
   WP_SYNC();
-  // R3: leaf sizes, then messages bottom-up, then offsets top-down
-  const u32 n_leaf = S.n_leaf;
-  for (u32 k = lane; k < n_leaf; k += 32) coop_size_leaf(S, cx, S.order[k], have_masks);
+  // R3: leaf sizes, then messages bottom-up, then offsets top-down - the messages one level at a time, straight from
+  // the queue: no lane visits a leaf or an entry of another depth
+  const u32 leaf_end = S.leaf_end;
+  for (u32 k = q_end + lane; k < leaf_end; k += 32) coop_size_leaf(S, cx, S.queue[k], have_masks);
   WP_SYNC();
   if (S.bail) return false;
   {
@@ -780,11 +782,9 @@ GGR_DEV bool coop_size_item(SH& S, const DecCtx& cx, u32 root_msg, u32 start, u3
     }
     WP_SYNC();
   }
-  const u32 maxd = S.max_depth;
-  for (u32 dd = 0; dd <= maxd; dd++) {
-    const u32 d = maxd - dd;
-    for (u32 i = lane; i < n; i += 32)
-      if (S.ent[i].depth == d && (S.ent[i].flags & CF_MSG)) coop_close_message(S, cx, i);
+  for (u32 l = nl; l-- > 0;) {
+    const u32 le = S.lvl[l + 1];
+    for (u32 i = S.lvl[l] + lane; i < le; i += 32) coop_close_message(S, cx, S.queue[i]);
     WP_SYNC();
   }
   *size = S.ent[0].size;
@@ -797,9 +797,9 @@ GGR_DEV bool coop_size_item(SH& S, const DecCtx& cx, u32 root_msg, u32 start, u3
     *tab_off = base;
   }
   if (!save) return true;
-  for (u32 d = 0; d <= maxd; d++) {
-    for (u32 i = lane; i < n; i += 32)
-      if (S.ent[i].depth == d && (S.ent[i].flags & CF_MSG)) coop_offsets_message(S, cx, i);
+  for (u32 l = 0; l < nl; l++) {
+    const u32 le = S.lvl[l + 1];
+    for (u32 i = S.lvl[l] + lane; i < le; i += 32) coop_offsets_message(S, cx, S.queue[i]);
     WP_SYNC();
   }
   // save the table: two 16-byte stores per entry
