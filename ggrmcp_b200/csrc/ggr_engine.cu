@@ -1,14 +1,9 @@
 // ggr_engine.cu - sm_90a kernels and the C ABI of include/ggrmcp_b200.h.
 //
-// Kernel plan (one item = one tools/call message, one thread per item, 128-thread blocks):
-//   request side : k_encode_parse  (pass A: JSON -> IR + exact size, block sums)
-//                  k_scan_blocks   (exclusive scan of the block sums, single block)
-//                  k_encode_emit   (block-local scan -> final offsets; pass B: IR -> wire bytes)
-//   reply side   : k_decode_size   (size pass over the wire bytes, block sums)
-//                  k_scan_blocks
-//                  k_decode_write  (block-local scan -> final offsets; write pass)
-//   error detail : k_diag_list, k_encode_parse (list mode), k_diag_locate, k_block_sums, k_scan_blocks, k_offsets, k_diag_write
-//                  (ggr_kernels_diag.cu: the failing items of a request batch, their error positions and texts)
+// Kernel plan: run_encode_kernels, run_decode_kernels, run_request_dev, run_diag_dev and run_wrap_dev list the stages of
+// the request side, the reply side, request bodies, error detail and result bodies, one launcher call each (ggr_kernels.h
+// states what each reads and writes).  Each fills its call's batch view once; the work lists (GgrWork) carry items from
+// the stage that fills one to the stages that run over it.
 // Items shard across GPUs by batch index on the caller's side (one engine per device); there is
 // no cross-GPU exchange on this path.
 #include <cuda_runtime.h>
@@ -95,17 +90,19 @@ __global__ void __launch_bounds__(256) k_route(long long n, const u64* __restric
 // none (the buffer is filled with 0xFF bytes before) - and the list-mode launches run over that list.  The list is
 // ordered by size class, largest first (five classes, each twice the one below): the warps of a launch are scheduled in
 // list order, and a wave that starts with the long items ends when the short ones of the last wave would have.
-// cnt: [0] threads of the list-mode launches, [1] small items, [2..6] items per class, [7..11] placed per class.
 // Request side (list != nullptr): splits the per-thread list into `small` and `spread`.
 // Reply side (list == nullptr): every item the warp-cooperative kernels left pending (mode) that is large.
 // phase 0 counts the classes, phase 1 places the items; what does not fit `cap_items` stays with the small / whole-batch pass.
+// cnt, the SP_HEAD words in front of the spread list: [SP_THREADS] threads of the list-mode launches, [SP_SMALL] small
+// items, five words from SP_CLASS items per class, five from SP_PLACED placed per class.
+enum : u32 { SP_THREADS = 0, SP_SMALL = 1, SP_CLASS = 2, SP_PLACED = 7, SP_HEAD = 16 };
 __global__ void __launch_bounds__(256) k_spread(int phase, long long n, const u64* __restrict__ in_off, u32 big_bytes, const u32* __restrict__ list,
                                                 const u32* __restrict__ list_n, const u32* __restrict__ mode, u32* __restrict__ small,
                                                 u32* __restrict__ spread, u32* __restrict__ cnt, u32 cap_items) {
   const long long t = (long long)blockIdx.x * 256 + threadIdx.x;
   if (phase == 1 && t == 0) {
-    const u32 total = cnt[2] + cnt[3] + cnt[4] + cnt[5] + cnt[6];
-    cnt[0] = (total < cap_items ? total : cap_items) * 32u;
+    const u32 total = cnt[SP_CLASS] + cnt[SP_CLASS + 1] + cnt[SP_CLASS + 2] + cnt[SP_CLASS + 3] + cnt[SP_CLASS + 4];
+    cnt[SP_THREADS] = (total < cap_items ? total : cap_items) * 32u;
   }
   long long i = n;
   if (list) {
@@ -116,23 +113,22 @@ __global__ void __launch_bounds__(256) k_spread(int phase, long long n, const u6
   if (i >= n) return;
   const u64 len = in_off[i + 1] - in_off[i];
   if (len < big_bytes) {
-    if (phase == 1 && small) small[atomicAdd(cnt + 1, 1u)] = (u32)i;
+    if (phase == 1 && small) small[atomicAdd(cnt + SP_SMALL, 1u)] = (u32)i;
     return;
   }
   u32 cls = 0;
   for (u64 x = len / big_bytes; x > 1 && cls < 4u; x >>= 1) cls++;
   if (phase == 0) {
-    atomicAdd(cnt + 2 + cls, 1u);
+    atomicAdd(cnt + SP_CLASS + cls, 1u);
     return;
   }
   u32 base = 0;
-  for (u32 c = cls + 1; c < 5u; c++) base += cnt[2 + c];
-  const u32 slot = base + atomicAdd(cnt + 7 + cls, 1u);
+  for (u32 c = cls + 1; c < 5u; c++) base += cnt[SP_CLASS + c];
+  const u32 slot = base + atomicAdd(cnt + SP_PLACED + cls, 1u);
   if (slot < cap_items) spread[(size_t)slot * 32] = (u32)i;
-  else if (small) small[atomicAdd(cnt + 1, 1u)] = (u32)i;
+  else if (small) small[atomicAdd(cnt + SP_SMALL, 1u)] = (u32)i;
 }
 
-// status / size of the items of a list (request bodies the lock-step parser cannot take)
 // the chunk's output size straight into mapped host memory: the host learns it from the stream's
 // event alone, without a copy that would queue behind other chunks' payloads on the copy engine
 __global__ void k_publish_total(const u64* __restrict__ src, const u64* __restrict__ src2, volatile u64* dst) {
@@ -141,6 +137,7 @@ __global__ void k_publish_total(const u64* __restrict__ src, const u64* __restri
   __threadfence_system();
 }
 
+// status / size of the items of a list (request bodies the lock-step parser cannot take)
 __global__ void __launch_bounds__(256) k_mark(const u32* __restrict__ list, const u32* __restrict__ list_n, i32* __restrict__ status,
                                               u32* __restrict__ size, u32* __restrict__ first, i32 value) {
   const u32 i = blockIdx.x * 256u + threadIdx.x;
@@ -310,35 +307,31 @@ static bool ensure(ggr_engine* e, DevBuf& b, size_t bytes) {
 }
 
 // The lock-step work lists of a call, in sc.pend: every list's header first (zeroed together), then n item indices per list.
-struct WorkList {
-  GgrList* h;
-  u32* item;
-};
 // request side: the router's lock-step items; what the walker leaves, after all its tiers (GGR_WALK=0: after the first
 // parser tier), after its first tier and after its second; the per-thread parser's items
 struct EncodeLists {
-  WorkList lockstep, walk_left, walk1_left, walk2_left, per_thread;
+  GgrWork lockstep, walk_left, walk1_left, walk2_left, per_thread;
 };
 // reply side: the router's lock-step items; what the first lock-step tier leaves
 struct DecodeLists {
-  WorkList lockstep, tier1_left;
+  GgrWork lockstep, tier1_left;
 };
 // request bodies: the router's lock-step items; what the first parser tier leaves; what neither tier can take
 struct BodyLists {
-  WorkList lockstep, tier1_left, rest;
+  GgrWork lockstep, tier1_left, rest;
 };
 // error detail of request items: the items to diagnose
 struct DiagLists {
-  WorkList failing;
+  GgrWork failing;
 };
 template <class Set>
 static constexpr int list_count() {
-  return sizeof(Set) / sizeof(WorkList);
+  return sizeof(Set) / sizeof(GgrWork);
 }
 template <class Set>
 static Set carve_lists(void* p, int64_t n) {
   Set set;
-  WorkList* w = reinterpret_cast<WorkList*>(&set);
+  GgrWork* w = reinterpret_cast<GgrWork*>(&set);
   GgrList* h = (GgrList*)p;
   u32* item = (u32*)(h + list_count<Set>());
   for (int k = 0; k < list_count<Set>(); k++) w[k] = {h + k, item + (size_t)k * n};
@@ -350,6 +343,71 @@ static bool make_lists(ggr_engine* e, DevBuf& pend, int64_t n, cudaStream_t st, 
   if (!ensure(e, pend, heads + list_count<Set>() * (size_t)n * 4) || !cuda_ok(e, cudaMemsetAsync(pend.p, 0, heads, st), "memset"))
     return false;
   *set = carve_lists<Set>(pend.p, n);
+  return true;
+}
+
+// The batch views of a call: its arguments and the scratch of sc, typed once (after sc's buffers are sized).
+template <class View>
+static View batch_view(const ggr_schema* s, Scratch& sc, int64_t n, const int32_t* msg_id, const uint8_t* in, const uint64_t* in_off,
+                       int32_t* status) {
+  View v;
+  v.blob = s->d_blob;
+  v.n_msgs = (u32)s->cs.msg_names.size();
+  v.n = n;
+  v.msg_id = msg_id;
+  v.in = in;
+  v.in_off = in_off;
+  v.size = (u32*)sc.size.p;
+  v.status = status;
+  v.sums = (u64*)sc.sums.p;
+  return v;
+}
+static GgrEncodeView encode_view(const ggr_schema* s, Scratch& sc, int64_t n, const int32_t* msg_id, const uint8_t* in,
+                                 const uint64_t* in_off, int32_t* status) {
+  GgrEncodeView v = batch_view<GgrEncodeView>(s, sc, n, msg_id, in, in_off, status);
+  v.ir = (u8*)sc.ir.p;
+  v.first = (u32*)sc.aux.p;
+  v.ioff = (u32*)sc.ioff.p;
+  v.nnodes = (u32*)sc.nn.p;
+  return v;
+}
+static GgrDecodeView decode_view(const ggr_schema* s, Scratch& sc, int64_t n, const int32_t* msg_id, const uint8_t* in,
+                                 const uint64_t* in_off, int32_t* status, uint32_t flags, u32 sort_cap, u32 pool_cap) {
+  GgrDecodeView v = batch_view<GgrDecodeView>(s, sc, n, msg_id, in, in_off, status);
+  v.flags = flags;
+  v.mode = (u32*)sc.aux.p;
+  v.sort_pool = sc.sortpool.p;
+  v.sort_cap = sort_cap;
+  v.tab = sc.ir.p;
+  v.nent = (u32*)sc.nn.p;
+  v.pool = sc.tabpool.p;
+  v.pool_cap = pool_cap;
+  v.tab_off = (u32*)sc.taboff.p;
+  return v;
+}
+
+// The large items of the per-thread kernels, a warp each (k_spread), in sc.spread: the counters, the spread list with room
+// for one item per spread_min bytes of input (at most GGR_SPREAD_CAP) and, on the request side, the small list.
+struct Spread {
+  const u32 *list, *list_n;    // the spread list and the thread count of its list-mode launches
+  const u32 *small, *small_n;  // request side: the rest of the per-thread list
+  unsigned blocks;             // of the list-mode launches
+};
+// Request side: split the per-thread list `from`.  Reply side (from null): the items the lock-step tiers left pending in mode.
+static bool spread_items(ggr_engine* e, const GgrLaunch& L, Scratch& sc, int64_t n, const uint64_t* in_off, uint64_t in_bytes,
+                         const GgrWork* from, const u32* mode, Spread* sp) {
+  size_t max_big = (size_t)(in_bytes / e->spread_min) + 1;
+  if (max_big > GGR_SPREAD_CAP) max_big = GGR_SPREAD_CAP;
+  const size_t slots = max_big * 32;
+  if (!ensure(e, sc.spread, (SP_HEAD + slots + (from ? (size_t)n : 0)) * 4)) return false;
+  u32* cnt = (u32*)sc.spread.p;
+  u32 *list = cnt + SP_HEAD, *small = from ? list + slots : nullptr;
+  if (!cuda_ok(e, cudaMemsetAsync(cnt, 0, SP_HEAD * 4, L.st), "memset") || !cuda_ok(e, cudaMemsetAsync(list, 0xFF, slots * 4, L.st), "memset"))
+    return false;
+  for (int phase = 0; phase < 2; phase++)
+    ggr_enqueue(L, k_spread, (unsigned)((n + 255) / 256), 256, 0, phase, n, in_off, e->spread_min, from ? from->item : nullptr,
+                from ? &from->h->n : nullptr, mode, small, list, cnt, (u32)max_big);
+  *sp = Spread{list, cnt + SP_THREADS, small, cnt + SP_SMALL, (unsigned)((slots + GGR_BLOCK - 1) / GGR_BLOCK)};
   return true;
 }
 
@@ -369,7 +427,8 @@ static int run_batch(ggr_engine* e, const ggr_schema* s, Scratch& sc, int64_t n,
   return cuda_ok(e, cudaGetLastError(), "kernel launch") ? GGR_SUCCESS : GGR_ERR_CUDA;
 }
 
-// GGR_POISON: after the last kernel of a device-buffer call, in stream order
+// GGR_POISON: after the last kernel of a device-buffer call, in stream order; not counted, so that a call's launch count
+// is the same with and without it
 static void poison_scratch(ggr_engine* e, Scratch& sc, cudaStream_t st) {
   if (!e || !e->poison) return;
   DevBuf* bufs[] = {&sc.ir, &sc.size, &sc.aux, &sc.sums, &sc.pend, &sc.ioff, &sc.nn, &sc.diag};
@@ -729,97 +788,64 @@ static int run_encode_kernels(ggr_engine* e, const ggr_schema* s, Scratch& sc, i
                               const uint8_t* in, const uint64_t* in_off, uint64_t in_bytes, uint8_t* out, uint64_t out_cap,
                               uint64_t* out_off, int32_t* status, uint32_t flags, cudaStream_t st) {
   const bool coop = e->use_coop_enc;
-  EncodeLists L;
+  EncodeLists W;
   if (!ensure(e, sc.ir, ggr_ir_bytes(in_bytes, n))) return GGR_ERR_CUDA;
-  if (coop && (!ensure(e, sc.ioff, ggr_ioff_bytes(in_bytes, n)) || !ensure(e, sc.nn, (size_t)n * 4) || !make_lists(e, sc.pend, n, st, &L) ||
+  if (coop && (!ensure(e, sc.ioff, ggr_ioff_bytes(in_bytes, n)) || !ensure(e, sc.nn, (size_t)n * 4) || !make_lists(e, sc.pend, n, st, &W) ||
                !cuda_ok(e, cudaMemsetAsync(sc.nn.p, 0, (size_t)n * 4, st), "memset")))
     return GGR_ERR_CUDA;
-  const u32 n_msgs = (u32)s->cs.msg_names.size();
+  const GgrLaunch L{st, e->sm_count, &e->launches};
+  const GgrEncodeView v = encode_view(s, sc, n, msg_id, in, in_off, status);
   const u32 frame = (flags & GGR_F_GRPC_FRAME) ? 5u : 0u;  // message header in front of every item
-  u8* ir = (u8*)sc.ir.p;
-  u32 *size = (u32*)sc.size.p, *first = (u32*)sc.aux.p, *ioff = (u32*)sc.ioff.p, *nn = (u32*)sc.nn.p;
-  u64* sums = (u64*)sc.sums.p;
   Prof prof(e, st);
   prof.mark();
   if (!coop) {
-    ggr_launch_encode_parse(st, (unsigned)nb, s->d_blob, n, n_msgs, msg_id, in, in_off, ir, size, first, status, sums, nullptr, nullptr);
-    e->launches += 1;
+    ggr_launch_encode_parse(L, v, (unsigned)nb);
     if (frame) {
-      ggr_launch_frame_sizes(st, n, size, status);
-      ggr_launch_block_sums(st, (unsigned)nb, n, size, sums);
-      e->launches += 2;
+      ggr_launch_frame_sizes(L, v);
+      ggr_launch_block_sums(L, (unsigned)nb, n, v.size, v.sums);
     }
     prof.span(P_ENCODE_PARSE);
   } else {
     // router: small (and oversized) items straight to the per-thread parser
-    k_route<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(n, in_off, e->min_json, 65000u - 16u, L.lockstep.item, &L.lockstep.h->n,
-                                                        L.per_thread.item, &L.per_thread.h->n, nullptr);
+    ggr_enqueue(L, k_route, (unsigned)((n + 255) / 256), 256, 0, n, in_off, e->min_json, 65000u - 16u, W.lockstep.item, &W.lockstep.h->n,
+                W.per_thread.item, &W.per_thread.h->n, nullptr);
     if (e->use_walk) {
-      // token index, value records, then types, sizes and offsets in three tiers, each over what the one before left: the
-      // second takes large items and the other leaf forms, the third (one warp per SM) thousands of values
-      ggr_launch_encode_tok2(st, n, in, in_off, ir, L.lockstep.item, L.lockstep.h, e->sm_count);
+      ggr_launch_encode_tok2(L, v, W.lockstep);
       prof.span(P_ENCODE_COOP_TOK);
-      ggr_launch_encode_place(st, n, in_off, ir, L.lockstep.item, L.lockstep.h, e->sm_count);
+      ggr_launch_encode_place(L, v, W.lockstep);
       prof.span(P_ENCODE_PLACE);
-      ggr_launch_encode_type(st, 0, n, s->d_blob, n_msgs, msg_id, in, in_off, ir, size, first, status, ioff, nn, L.lockstep.item, L.lockstep.h,
-                             L.walk1_left.item, L.walk1_left.h, e->sm_count);
-      ggr_launch_encode_type(st, 1, n, s->d_blob, n_msgs, msg_id, in, in_off, ir, size, first, status, ioff, nn, L.walk1_left.item,
-                             L.walk1_left.h, L.walk2_left.item, L.walk2_left.h, e->sm_count);
-      ggr_launch_encode_type(st, 2, n, s->d_blob, n_msgs, msg_id, in, in_off, ir, size, first, status, ioff, nn, L.walk2_left.item,
-                             L.walk2_left.h, L.walk_left.item, L.walk_left.h, e->sm_count);
+      ggr_launch_encode_type(L, v, 0, W.lockstep, W.walk1_left);
+      ggr_launch_encode_type(L, v, 1, W.walk1_left, W.walk2_left);
+      ggr_launch_encode_type(L, v, 2, W.walk2_left, W.walk_left);
       prof.span(P_ENCODE_TYPE);
-      e->launches += 6;
     } else {
-      ggr_launch_encode_coop_tok(st, n, in, in_off, ir, L.lockstep.item, L.lockstep.h, e->sm_count);
+      ggr_launch_encode_coop_tok(L, v, W.lockstep);
       prof.span(P_ENCODE_COOP_TOK);
-      ggr_launch_encode_coop_parse(st, 0, n, s->d_blob, n_msgs, msg_id, in, in_off, ir, size, first, status, ioff, nn, L.lockstep.item,
-                                   L.lockstep.h, L.walk_left.item, L.walk_left.h, e->sm_count, nullptr, nullptr, -1);
-      e->launches += 3;
+      ggr_launch_encode_coop_parse(L, v, 0, W.lockstep, W.walk_left);
     }
-    ggr_launch_encode_coop_parse(st, 1, n, s->d_blob, n_msgs, msg_id, in, in_off, ir, size, first, status, ioff, nn, L.walk_left.item,
-                                 L.walk_left.h, L.per_thread.item, L.per_thread.h, e->sm_count, nullptr, nullptr, -1);
-    e->launches += 1;
+    ggr_launch_encode_coop_parse(L, v, 1, W.walk_left, W.per_thread);
     prof.span(P_ENCODE_COOP_PARSE);
     if (e->spread_min) {
-      // the per-thread list, split: small items 32 to a warp, large ones a warp each (k_spread)
-      size_t max_big = (size_t)(in_bytes / e->spread_min) + 1;  // items of at least spread_min bytes
-      if (max_big > GGR_SPREAD_CAP) max_big = GGR_SPREAD_CAP;
-      if (!ensure(e, sc.spread, (max_big * 32 + (size_t)n) * 4 + 64)) return GGR_ERR_CUDA;
-      u32* sp_cnt = (u32*)sc.spread.p;
-      u32* sp_list = sp_cnt + 16;
-      u32* sp_small = sp_list + max_big * 32;
-      if (!cuda_ok(e, cudaMemsetAsync(sp_cnt, 0, 64, st), "memset") || !cuda_ok(e, cudaMemsetAsync(sp_list, 0xFF, max_big * 32 * 4, st), "memset"))
-        return GGR_ERR_CUDA;
-      for (int phase = 0; phase < 2; phase++)
-        k_spread<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(phase, n, in_off, e->spread_min, L.per_thread.item, &L.per_thread.h->n, nullptr,
-                                                             sp_small, sp_list, sp_cnt, (u32)max_big);
-      ggr_launch_encode_parse(st, (unsigned)((max_big * 32 + GGR_BLOCK - 1) / GGR_BLOCK), s->d_blob, n, n_msgs, msg_id, in, in_off, ir, size,
-                              first, status, sums, sp_list, sp_cnt);
-      ggr_launch_encode_parse(st, (unsigned)nb, s->d_blob, n, n_msgs, msg_id, in, in_off, ir, size, first, status, sums, sp_small, sp_cnt + 1);
-      e->launches += 4;
+      // the per-thread list, split: small items 32 to a warp, large ones a warp each
+      Spread sp;
+      if (!spread_items(e, L, sc, n, in_off, in_bytes, &W.per_thread, nullptr, &sp)) return GGR_ERR_CUDA;
+      ggr_launch_encode_parse(L, v, sp.blocks, sp.list, sp.list_n);
+      ggr_launch_encode_parse(L, v, (unsigned)nb, sp.small, sp.small_n);
     } else {
-      ggr_launch_encode_parse(st, (unsigned)nb, s->d_blob, n, n_msgs, msg_id, in, in_off, ir, size, first, status, sums, L.per_thread.item,
-                              &L.per_thread.h->n);
-      e->launches += 1;
+      ggr_launch_encode_parse(L, v, (unsigned)nb, W.per_thread.item, &W.per_thread.h->n);
     }
     prof.span(P_ENCODE_PARSE);
-    if (frame) {
-      ggr_launch_frame_sizes(st, n, size, status);
-      e->launches += 1;
-    }
-    ggr_launch_block_sums(st, (unsigned)nb, n, size, sums);
-    e->launches += 1;
+    if (frame) ggr_launch_frame_sizes(L, v);
+    ggr_launch_block_sums(L, (unsigned)nb, n, v.size, v.sums);
     prof.span(P_ENCODE_BLOCK_SUMS);
   }
-  k_scan_blocks<<<1, 1024, 0, st>>>(sums, nb, out_off + n);
+  ggr_enqueue(L, k_scan_blocks, 1, 1024, 0, v.sums, nb, out_off + n);
   prof.span(P_ENCODE_SCAN);
-  ggr_launch_encode_emit(st, (unsigned)nb, n, in, in_off, ir, size, first, status, sums, out, out_cap, out_off, coop ? nn : nullptr, frame);
+  ggr_launch_encode_emit(L, v, (unsigned)nb, out, out_cap, out_off, coop ? v.nnodes : nullptr, frame);
   prof.span(P_ENCODE_EMIT);
-  e->launches += 2;
   if (coop) {
-    ggr_launch_encode_coop_emit(st, n, in, in_off, ir, ioff, nn, size, status, out, out_off, e->sm_count, L.lockstep.item, L.lockstep.h, frame);
+    ggr_launch_encode_coop_emit(L, v, W.lockstep, out, out_off, frame);
     prof.span(P_ENCODE_COOP_EMIT);
-    e->launches += 1;
   }
   return GGR_SUCCESS;
 }
@@ -830,7 +856,6 @@ static int run_decode_kernels(ggr_engine* e, const ggr_schema* s, Scratch& sc, i
                               const uint8_t* in, const uint64_t* in_off, uint64_t in_bytes, uint8_t* out, uint64_t out_cap,
                               uint64_t* out_off, int32_t* status, uint32_t flags, cudaStream_t st) {
   const bool coop = e->use_coop;
-  const u32 n_msgs = (u32)s->cs.msg_names.size();
   Prof prof(e, st);
   prof.mark();
   // a map entry takes at least 4 bytes of wire; both passes sort, the fast walk may give way to the slow one
@@ -838,61 +863,39 @@ static int run_decode_kernels(ggr_engine* e, const ggr_schema* s, Scratch& sc, i
   const uint32_t sort_cap = (uint32_t)(want_recs > 0x3FFFFFFFull ? 0x3FFFFFFFull : want_recs);
   if (!ensure(e, sc.sortpool, (size_t)sort_cap * 16 + 16)) return GGR_ERR_CUDA;
   if (!cuda_ok(e, cudaMemsetAsync(sc.sortpool.p, 0, 16, st), "memset")) return GGR_ERR_CUDA;
-  DecodeLists L;
+  // second tier's tables: a field occurrence takes at least 2 bytes of wire; the pool is capped at 4 M entries (128 MB)
+  const uint64_t want_ent = in_bytes / 2 + 4096;
+  const uint32_t pool_cap = (uint32_t)(want_ent > (4ull << 20) ? (4ull << 20) : want_ent);
+  DecodeLists W;
+  if (coop && (!ensure(e, sc.ir, ggr_decode_coop_table_bytes(n)) || !ensure(e, sc.nn, (size_t)n * 4) || !make_lists(e, sc.pend, n, st, &W) ||
+               !ensure(e, sc.tabpool, (size_t)pool_cap * 32 + 32) || !ensure(e, sc.taboff, (size_t)n * 4) ||
+               !cuda_ok(e, cudaMemsetAsync(sc.tabpool.p, 0, 32, st), "memset")))
+    return GGR_ERR_CUDA;
+  const GgrLaunch L{st, e->sm_count, &e->launches};
+  const GgrDecodeView v = decode_view(s, sc, n, msg_id, in, in_off, status, flags, sort_cap, pool_cap);
   if (coop) {
-    // second tier's tables: a field occurrence takes at least 2 bytes of wire; the pool is capped at 4 M entries (128 MB)
-    const uint64_t want_ent = in_bytes / 2 + 4096;
-    const uint32_t pool_cap = (uint32_t)(want_ent > (4ull << 20) ? (4ull << 20) : want_ent);
-    if (!ensure(e, sc.ir, ggr_decode_coop_table_bytes(n)) || !ensure(e, sc.nn, (size_t)n * 4) || !make_lists(e, sc.pend, n, st, &L) ||
-        !ensure(e, sc.tabpool, (size_t)pool_cap * 32 + 32) || !ensure(e, sc.taboff, (size_t)n * 4) ||
-        !cuda_ok(e, cudaMemsetAsync(sc.tabpool.p, 0, 32, st), "memset"))
-      return GGR_ERR_CUDA;
-    k_route<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(n, in_off, e->min_wire, 0x3FFFFF00u, L.lockstep.item, &L.lockstep.h->n, nullptr,
-                                                        nullptr, (u32*)sc.aux.p);
-    ggr_launch_decode_coop_size(st, n, s->d_blob, n_msgs, msg_id, in, in_off, flags, (u32*)sc.size.p, (u32*)sc.aux.p, status, sc.ir.p,
-                                (u32*)sc.nn.p, e->sm_count, L.lockstep.item, L.lockstep.h, L.tier1_left.item, L.tier1_left.h, sc.tabpool.p,
-                                pool_cap, (u32*)sc.taboff.p);
-    e->launches += 3;
+    ggr_enqueue(L, k_route, (unsigned)((n + 255) / 256), 256, 0, n, in_off, e->min_wire, 0x3FFFFF00u, W.lockstep.item, &W.lockstep.h->n,
+                nullptr, nullptr, v.mode);
+    ggr_launch_decode_coop_size(L, v, W.lockstep, W.tier1_left);
     prof.span(P_DECODE_COOP_SIZE);
   }
-  // large items the lock-step kernels left: a warp each (k_spread), sized before and written after the pass over the batch
+  // large items the lock-step kernels left: a warp each, sized before and written after the pass over the batch
   const bool spread = coop && e->spread_min != 0;
-  size_t max_big = spread ? (size_t)(in_bytes / e->spread_min) + 1 : 0;
-  if (max_big > GGR_SPREAD_CAP) max_big = GGR_SPREAD_CAP;
-  const unsigned spread_blocks = (unsigned)((max_big * 32 + GGR_BLOCK - 1) / GGR_BLOCK);
-  u32* sp_cnt = nullptr;
+  Spread sp;
   if (spread) {
-    if (!ensure(e, sc.spread, max_big * 32 * 4 + 64)) return GGR_ERR_CUDA;
-    sp_cnt = (u32*)sc.spread.p;
-    if (!cuda_ok(e, cudaMemsetAsync(sp_cnt, 0, 64, st), "memset") || !cuda_ok(e, cudaMemsetAsync(sp_cnt + 16, 0xFF, max_big * 32 * 4, st), "memset"))
-      return GGR_ERR_CUDA;
-    for (int phase = 0; phase < 2; phase++)
-      k_spread<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(phase, n, in_off, e->spread_min, nullptr, nullptr, (const u32*)sc.aux.p, nullptr,
-                                                           sp_cnt + 16, sp_cnt, (u32)max_big);
-    ggr_launch_decode_size(st, spread_blocks, s->d_blob, n, n_msgs, msg_id, in, in_off, flags, (u32*)sc.size.p, (u32*)sc.aux.p, status,
-                           (u64*)sc.sums.p, 1, sc.sortpool.p, sort_cap, sp_cnt + 16, sp_cnt);
-    e->launches += 3;
+    if (!spread_items(e, L, sc, n, in_off, in_bytes, nullptr, v.mode, &sp)) return GGR_ERR_CUDA;
+    ggr_launch_decode_size(L, v, sp.blocks, 1, sp.list, sp.list_n);
   }
-  ggr_launch_decode_size(st, (unsigned)nb, s->d_blob, n, n_msgs, msg_id, in, in_off, flags, (u32*)sc.size.p, (u32*)sc.aux.p, status,
-                         (u64*)sc.sums.p, coop ? 1 : 0, sc.sortpool.p, sort_cap);
+  ggr_launch_decode_size(L, v, (unsigned)nb, coop ? 1 : 0);
   prof.span(P_DECODE_SIZE);
-  k_scan_blocks<<<1, 1024, 0, st>>>((u64*)sc.sums.p, nb, out_off + n);
+  ggr_enqueue(L, k_scan_blocks, 1, 1024, 0, v.sums, nb, out_off + n);
   prof.span(P_DECODE_SCAN);
-  ggr_launch_decode_write(st, (unsigned)nb, s->d_blob, n, msg_id, in, in_off, flags, (const u32*)sc.size.p, (const u32*)sc.aux.p, status,
-                          (const u64*)sc.sums.p, out, out_cap, out_off, sc.sortpool.p, sort_cap);
-  e->launches += 3;
-  if (spread) {
-    ggr_launch_decode_write(st, spread_blocks, s->d_blob, n, msg_id, in, in_off, flags, (const u32*)sc.size.p, (const u32*)sc.aux.p, status,
-                            (const u64*)sc.sums.p, out, out_cap, out_off, sc.sortpool.p, sort_cap, sp_cnt + 16, sp_cnt);
-    e->launches += 1;
-  }
+  ggr_launch_decode_write(L, v, (unsigned)nb, out, out_cap, out_off);
+  if (spread) ggr_launch_decode_write(L, v, sp.blocks, out, out_cap, out_off, sp.list, sp.list_n);
   prof.span(P_DECODE_WRITE);
   if (coop) {
-    ggr_launch_decode_coop_write(st, n, s->d_blob, in, in_off, flags, (const u32*)sc.size.p, (const u32*)sc.aux.p, status, sc.ir.p,
-                                 (const u32*)sc.nn.p, out, out_off, e->sm_count, L.lockstep.item, L.lockstep.h, sc.tabpool.p,
-                                 (const u32*)sc.taboff.p);
+    ggr_launch_decode_coop_write(L, v, W.lockstep, out, out_off);
     prof.span(P_DECODE_COOP_WRITE);
-    e->launches += 1;
   }
   return GGR_SUCCESS;
 }
@@ -918,24 +921,27 @@ static int run_diag_dev(ggr_engine* e, const ggr_schema* s, Scratch& sc, int64_t
                         uint64_t text_cap, uint64_t* text_off, int32_t* parse_status, cudaStream_t st) {
   const bool have_args = msg_id && in && in_off && err_pos && err_len && (text || !text_cap);
   const int rc = run_batch(e, s, sc, n, have_args, in, nullptr, text_off, st, [&](long long nb) {
-    DiagLists L;
-    if (!ensure(e, sc.ir, ggr_ir_bytes(in_bytes, n)) || !ensure(e, sc.diag, (size_t)n * 20) || !make_lists(e, sc.pend, n, st, &L))
+    DiagLists W;
+    if (!ensure(e, sc.ir, ggr_ir_bytes(in_bytes, n)) || !ensure(e, sc.diag, (size_t)n * 20) || !make_lists(e, sc.pend, n, st, &W))
       return GGR_ERR_CUDA;
-    u32* d = (u32*)sc.diag.p;
-    u32 *parse_pos = d + n, *text_len = d + 2 * n, *line = d + 3 * n, *col = d + 4 * n;
-    if (!parse_status) parse_status = (i32*)d;
-    u64* sums = (u64*)sc.sums.p;
-    ggr_launch_diag_list(st, n, status, L.failing.item, L.failing.h, err_pos, err_len, text_len);
-    ggr_launch_encode_parse(st, (unsigned)nb, s->d_blob, n, (u32)s->cs.msg_names.size(), msg_id, in, in_off, (u8*)sc.ir.p, (u32*)sc.size.p,
-                            (u32*)sc.aux.p, parse_status, sums, L.failing.item, &L.failing.h->n, parse_pos);
-    ggr_launch_diag_locate(st, n, in, in_off, parse_status, parse_pos, L.failing.item, L.failing.h, err_pos, err_len, text_len, line, col,
-                           e->sm_count);
-    ggr_launch_block_sums(st, (unsigned)nb, n, text_len, sums);
-    k_scan_blocks<<<1, 1024, 0, st>>>(sums, nb, text_off + n);
-    ggr_launch_offsets(st, (unsigned)nb, n, text_len, sums, text_off);
-    ggr_launch_diag_write(st, n, in, in_off, parse_status, L.failing.item, L.failing.h, err_pos, err_len, text_len, line, col, text, text_cap,
-                          text_off, e->sm_count);
-    e->launches += 7;
+    const GgrLaunch L{st, e->sm_count, &e->launches};
+    u32* w = (u32*)sc.diag.p;  // five words per item
+    GgrDiagView d;
+    d.parse_status = parse_status ? parse_status : (i32*)w;
+    d.parse_pos = w + n;
+    d.err_pos = err_pos;
+    d.err_len = err_len;
+    d.text_len = w + 2 * n;
+    d.line = w + 3 * n;
+    d.col = w + 4 * n;
+    const GgrEncodeView v = encode_view(s, sc, n, msg_id, in, in_off, d.parse_status);
+    ggr_launch_diag_list(L, n, status, W.failing, d);
+    ggr_launch_encode_parse(L, v, (unsigned)nb, W.failing.item, &W.failing.h->n, d.parse_pos);
+    ggr_launch_diag_locate(L, v, W.failing, d);
+    ggr_launch_block_sums(L, (unsigned)nb, n, d.text_len, v.sums);
+    ggr_enqueue(L, k_scan_blocks, 1, 1024, 0, v.sums, nb, text_off + n);
+    ggr_launch_offsets(L, (unsigned)nb, n, d.text_len, v.sums, text_off);
+    ggr_launch_diag_write(L, v, W.failing, d, text, text_cap, text_off);
     return GGR_SUCCESS;
   });
   poison_scratch(e, sc, st);
@@ -966,28 +972,25 @@ static int run_request_dev(ggr_engine* e, const ggr_schema* s, Scratch& sc, int6
                            int32_t* status, cudaStream_t st) {
   const bool have_args = in && in_off && out_off && status && method && id_span;
   return run_batch(e, s, sc, n, have_args, in, out, out_off, st, [&](long long nb) {
-    BodyLists L;
+    BodyLists W;
     if (!ensure(e, sc.ir, ggr_ir_bytes(in_bytes, n)) || !ensure(e, sc.ioff, ggr_ioff_bytes(in_bytes, n)) || !ensure(e, sc.nn, (size_t)n * 4) ||
-        !make_lists(e, sc.pend, n, st, &L) || !cuda_ok(e, cudaMemsetAsync(sc.nn.p, 0, (size_t)n * 4, st), "memset"))
+        !make_lists(e, sc.pend, n, st, &W) || !cuda_ok(e, cudaMemsetAsync(sc.nn.p, 0, (size_t)n * 4, st), "memset"))
       return GGR_ERR_CUDA;
-    const u32 n_msgs = (u32)s->cs.msg_names.size();
-    u8* ir = (u8*)sc.ir.p;
-    u32 *size = (u32*)sc.size.p, *first = (u32*)sc.aux.p, *ioff = (u32*)sc.ioff.p, *nn = (u32*)sc.nn.p;
-    u64* sums = (u64*)sc.sums.p;
+    const GgrLaunch L{st, e->sm_count, &e->launches};
+    GgrEncodeView v = encode_view(s, sc, n, nullptr, in, in_off, status);
+    v.method = method;
+    v.id_span = id_span;
     // bodies above the parser's input limit cannot be taken
-    k_route<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(n, in_off, 0u, 65000u - 16u, L.lockstep.item, &L.lockstep.h->n, L.rest.item,
-                                                        &L.rest.h->n, nullptr);
-    ggr_launch_encode_coop_tok(st, n, in, in_off, ir, L.lockstep.item, L.lockstep.h, e->sm_count);
-    ggr_launch_encode_coop_parse(st, 0, n, s->d_blob, n_msgs, nullptr, in, in_off, ir, size, first, status, ioff, nn, L.lockstep.item,
-                                 L.lockstep.h, L.tier1_left.item, L.tier1_left.h, e->sm_count, method, id_span, -1);
-    ggr_launch_encode_coop_parse(st, 1, n, s->d_blob, n_msgs, nullptr, in, in_off, ir, size, first, status, ioff, nn, L.tier1_left.item,
-                                 L.tier1_left.h, L.rest.item, L.rest.h, e->sm_count, method, id_span, GGR_ST_UNSUPPORTED);
-    k_mark<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(L.rest.item, &L.rest.h->n, status, size, first, GGR_ST_UNSUPPORTED);
-    ggr_launch_block_sums(st, (unsigned)nb, n, size, sums);
-    k_scan_blocks<<<1, 1024, 0, st>>>(sums, nb, out_off + n);
-    ggr_launch_encode_emit(st, (unsigned)nb, n, in, in_off, ir, size, first, status, sums, out, out_cap, out_off, nn, 0);
-    ggr_launch_encode_coop_emit(st, n, in, in_off, ir, ioff, nn, size, status, out, out_off, e->sm_count, L.lockstep.item, L.lockstep.h, 0);
-    e->launches += 9;
+    ggr_enqueue(L, k_route, (unsigned)((n + 255) / 256), 256, 0, n, in_off, 0u, 65000u - 16u, W.lockstep.item, &W.lockstep.h->n, W.rest.item,
+                &W.rest.h->n, nullptr);
+    ggr_launch_encode_coop_tok(L, v, W.lockstep);
+    ggr_launch_encode_coop_parse(L, v, 0, W.lockstep, W.tier1_left);
+    ggr_launch_encode_coop_parse(L, v, 1, W.tier1_left, W.rest, GGR_ST_UNSUPPORTED);
+    ggr_enqueue(L, k_mark, (unsigned)((n + 255) / 256), 256, 0, W.rest.item, &W.rest.h->n, v.status, v.size, v.first, GGR_ST_UNSUPPORTED);
+    ggr_launch_block_sums(L, (unsigned)nb, n, v.size, v.sums);
+    ggr_enqueue(L, k_scan_blocks, 1, 1024, 0, v.sums, nb, out_off + n);
+    ggr_launch_encode_emit(L, v, (unsigned)nb, out, out_cap, out_off, v.nnodes, 0);
+    ggr_launch_encode_coop_emit(L, v, W.lockstep, out, out_off, 0);
     return GGR_SUCCESS;
   });
 }
@@ -1001,16 +1004,19 @@ static int run_wrap_dev(ggr_engine* e, const ggr_schema* s, Scratch& sc, int64_t
   if (n == 0) return run_dev(e, s, sc, false, n, msg_id, in, in_off, in_bytes, out, out_cap, out_off, status, flags, st);
   if (!ensure(e, sc.wtext, (size_t)out_cap + 64) || !ensure(e, sc.woff, (size_t)(n + 1) * 8) || !ensure(e, sc.wsize, (size_t)n * 4))
     return GGR_ERR_CUDA;
-  int rc = run_dev(e, s, sc, false, n, msg_id, in, in_off, in_bytes, (uint8_t*)sc.wtext.p, out_cap, (uint64_t*)sc.woff.p, status, flags, st);
+  u8* text = (u8*)sc.wtext.p;
+  u64* text_off = (u64*)sc.woff.p;
+  u32* size = (u32*)sc.wsize.p;
+  const int rc = run_dev(e, s, sc, false, n, msg_id, in, in_off, in_bytes, text, out_cap, text_off, status, flags, st);
   if (rc != GGR_SUCCESS) return rc;
+  const GgrLaunch L{st, e->sm_count, &e->launches};
   const long long nb = (n + GGR_BLOCK - 1) / GGR_BLOCK;
-  ggr_launch_wrap_size(st, n, (const uint8_t*)sc.wtext.p, (const uint64_t*)sc.woff.p, status, ids_off, (u32*)sc.wsize.p, e->sm_count);
-  ggr_launch_block_sums(st, (unsigned)nb, n, (const u32*)sc.wsize.p, (u64*)sc.sums.p);
-  k_scan_blocks<<<1, 1024, 0, st>>>((u64*)sc.sums.p, nb, out_off + n);
-  ggr_launch_offsets(st, (unsigned)nb, n, (const u32*)sc.wsize.p, (const u64*)sc.sums.p, out_off);
-  ggr_launch_wrap_write(st, n, (const uint8_t*)sc.wtext.p, (const uint64_t*)sc.woff.p, status, ids, ids_off, (const u32*)sc.wsize.p, out,
-                        out_cap, out_off, e->sm_count);
-  e->launches += 5;
+  u64* sums = (u64*)sc.sums.p;  // sized by run_dev
+  ggr_launch_wrap_size(L, n, text, text_off, status, ids_off, size);
+  ggr_launch_block_sums(L, (unsigned)nb, n, size, sums);
+  ggr_enqueue(L, k_scan_blocks, 1, 1024, 0, sums, nb, out_off + n);
+  ggr_launch_offsets(L, (unsigned)nb, n, size, sums, out_off);
+  ggr_launch_wrap_write(L, n, text, text_off, status, ids, ids_off, size, out, out_cap, out_off);
   return cuda_ok(e, cudaGetLastError(), "kernel launch") ? GGR_SUCCESS : GGR_ERR_CUDA;
 }
 
@@ -1108,9 +1114,8 @@ static int chunk_issue(ggr_engine* e, const ggr_schema* s, Slot& sl, bool encode
   if (rc != GGR_SUCCESS) return rc;
   if (!cuda_ok(e, cudaEventRecord(sl.ev_k, st), "event")) return GGR_ERR_CUDA;
   if (tr) cudaEventRecord(tr[1], st);
-  k_publish_total<<<1, 1, 0, st>>>((const u64*)sl.d_out_off.p + j.nc, ids ? (const u64*)sl.sc.woff.p + j.nc : nullptr,
-                                   (volatile u64*)sl.d_total_alias);
-  e->launches++;
+  ggr_enqueue(GgrLaunch{st, e->sm_count, &e->launches}, k_publish_total, 1, 1, 0, (const u64*)sl.d_out_off.p + j.nc,
+              ids ? (const u64*)sl.sc.woff.p + j.nc : nullptr, (volatile u64*)sl.d_total_alias);
   if (!cuda_ok(e, cudaGetLastError(), "k_publish_total") || !cuda_ok(e, cudaEventRecord(sl.ready, st), "event")) return GGR_ERR_CUDA;
   return GGR_SUCCESS;
 }

@@ -131,27 +131,21 @@ int ggr_decode_coop_init() {
                                        (int)(sizeof(CoopStage) * COOP_WRITE_WARPS));
   return (a == cudaSuccess && b == cudaSuccess) ? 0 : -1;
 }
-void ggr_launch_decode_coop_size(cudaStream_t st, long long n, const uint8_t* blob, uint32_t n_msgs, const int32_t* msg_id,
-                                 const uint8_t* in, const uint64_t* in_off, uint32_t flags, uint32_t* size, uint32_t* mode,
-                                 int32_t* status, void* tab, uint32_t* nent, int sm_count, const uint32_t* list,
-                                 const GgrList* list_h, uint32_t* pending, GgrList* pending_h, void* pool, uint32_t pool_cap,
-                                 uint32_t* tab_off) {
-  // first tier over the router's list; second tier (tables of thousands of entries, one warp per SM, saved in the pool; its
-  // list length lives on the device) over what the first left.  Resident blocks of the first tier: what the entry tables
-  // in shared memory allow (6 with 224 entries per warp, 4 with 320)
+void ggr_launch_decode_coop_size(const GgrLaunch& L, const GgrDecodeView& v, GgrWork in, GgrWork left) {
+  // resident blocks of the first tier: what the entry tables in shared memory allow (6 with 224 entries per warp, 4 with 320);
+  // the second (tables of thousands of entries) runs one warp per SM, its list length lives on the device
   static const int resident = ggr_resident_blocks((const void*)k_decode_coop_size<CoopShared, COOP_WARPS>, COOP_WARPS * 32,
                                                   coop_smem_bytes<CoopShared, COOP_WARPS>(), 4);
-  k_decode_coop_size<CoopShared, COOP_WARPS><<<ggr_persistent_grid(n, COOP_WARPS, sm_count, resident), COOP_WARPS * 32, coop_smem_bytes<CoopShared, COOP_WARPS>(), st>>>(
-      blob, n, n_msgs, msg_id, in, (const u64*)in_off, flags, size, mode, status, (U4*)tab, nent, list, list_h, pending, pending_h, nullptr, 0u, nullptr);
-  k_decode_coop_size<CoopSharedBig, 1><<<(unsigned)sm_count, 32, coop_smem_bytes<CoopSharedBig, 1>(), st>>>(
-      blob, n, n_msgs, msg_id, in, (const u64*)in_off, flags, size, mode, status, (U4*)tab, nent, pending, pending_h, nullptr, nullptr, (U4*)pool, pool_cap,
-      tab_off);
+  ggr_enqueue(L, k_decode_coop_size<CoopShared, COOP_WARPS>, ggr_persistent_grid(v.n, COOP_WARPS, L.sm_count, resident), COOP_WARPS * 32,
+              coop_smem_bytes<CoopShared, COOP_WARPS>(), v.blob, v.n, v.n_msgs, v.msg_id, v.in, v.in_off, v.flags, v.size, v.mode, v.status,
+              (U4*)v.tab, v.nent, in.item, in.h, left.item, left.h, nullptr, 0u, nullptr);
+  ggr_enqueue(L, k_decode_coop_size<CoopSharedBig, 1>, (unsigned)L.sm_count, 32, coop_smem_bytes<CoopSharedBig, 1>(), v.blob, v.n, v.n_msgs,
+              v.msg_id, v.in, v.in_off, v.flags, v.size, v.mode, v.status, (U4*)v.tab, v.nent, left.item, left.h, nullptr, nullptr,
+              (U4*)v.pool, v.pool_cap, v.tab_off);
 }
-void ggr_launch_decode_coop_write(cudaStream_t st, long long n, const uint8_t* blob, const uint8_t* in, const uint64_t* in_off,
-                                  uint32_t flags, const uint32_t* size, const uint32_t* mode, int32_t* status, const void* tab,
-                                  const uint32_t* nent, uint8_t* out, const uint64_t* out_off, int sm_count,
-                                  const uint32_t* list, const GgrList* list_h, const void* pool, const uint32_t* tab_off) {
+void ggr_launch_decode_coop_write(const GgrLaunch& L, const GgrDecodeView& v, GgrWork in, uint8_t* out, const uint64_t* out_off) {
   static const int resident = ggr_resident_blocks((const void*)k_decode_coop_write, COOP_WRITE_WARPS * 32, sizeof(CoopStage) * COOP_WRITE_WARPS, 6);
-  k_decode_coop_write<<<ggr_persistent_grid(n, COOP_WRITE_WARPS, sm_count, resident), COOP_WRITE_WARPS * 32, sizeof(CoopStage) * COOP_WRITE_WARPS, st>>>(
-      blob, n, in, (const u64*)in_off, flags, size, mode, status, (const U4*)tab, nent, out, (const u64*)out_off, list, list_h, (const U4*)pool, tab_off);
+  ggr_enqueue(L, k_decode_coop_write, ggr_persistent_grid(v.n, COOP_WRITE_WARPS, L.sm_count, resident), COOP_WRITE_WARPS * 32,
+              sizeof(CoopStage) * COOP_WRITE_WARPS, v.blob, v.n, v.in, v.in_off, v.flags, v.size, v.mode, v.status, (const U4*)v.tab, v.nent, out,
+              out_off, in.item, in.h, (const U4*)v.pool, v.tab_off);
 }

@@ -151,47 +151,34 @@ int ggr_encode_coop_init() {
 }
 
 template <class SH, bool ENV, bool PRE>
-static void ce_launch(cudaStream_t st, unsigned nb, long long n, const uint8_t* blob, uint32_t n_msgs, const int32_t* msg_id,
-                      const uint8_t* in, const uint64_t* in_off, uint8_t* ir, uint32_t* size, uint32_t* first, int32_t* status,
-                      uint32_t* ioff, uint32_t* nnodes, const uint32_t* list, const GgrList* list_h, uint32_t* pending,
-                      GgrList* pending_h, int32_t* method, uint32_t* id_span, int32_t final_status) {
-  k_encode_coop_parse<SH, ENV, PRE><<<nb, CE_WARPS * 32, ce_smem_bytes<SH>(), st>>>(
-      blob, n, n_msgs, msg_id, in, (const u64*)in_off, ir, size, first, status, ioff, nnodes, list, list_h, pending, pending_h, method,
-      id_span, final_status);
+static void ce_launch(const GgrLaunch& L, unsigned nb, const GgrEncodeView& v, GgrWork in, GgrWork left, int32_t final_status) {
+  ggr_enqueue(L, k_encode_coop_parse<SH, ENV, PRE>, nb, CE_WARPS * 32, ce_smem_bytes<SH>(), v.blob, v.n, v.n_msgs, v.msg_id, v.in, v.in_off,
+              v.ir, v.size, v.first, v.status, v.ioff, v.nnodes, in.item, in.h, left.item, left.h, v.method, v.id_span, final_status);
 }
 
-// token index of tier 1 (before ggr_launch_encode_coop_parse with tier 0, same list)
-void ggr_launch_encode_coop_tok(cudaStream_t st, long long n, const uint8_t* in, const uint64_t* in_off, uint8_t* ir,
-                                const uint32_t* list, const GgrList* list_h, int sm_count) {
-  k_encode_coop_tok<<<ggr_persistent_grid(n, CE_WARPS, sm_count, CE_TOK_BLOCKS), CE_WARPS * 32, ce_smem_bytes<CoopTok>(), st>>>(
-      n, in, (const u64*)in_off, ir, list, list_h);
+void ggr_launch_encode_coop_tok(const GgrLaunch& L, const GgrEncodeView& v, GgrWork in) {
+  ggr_enqueue(L, k_encode_coop_tok, ggr_persistent_grid(v.n, CE_WARPS, L.sm_count, CE_TOK_BLOCKS), CE_WARPS * 32, ce_smem_bytes<CoopTok>(),
+              v.n, v.in, v.in_off, v.ir, in.item, in.h);
 }
 
-void ggr_launch_encode_coop_parse(cudaStream_t st, int tier, long long n, const uint8_t* blob, uint32_t n_msgs,
-                                  const int32_t* msg_id, const uint8_t* in, const uint64_t* in_off, uint8_t* ir, uint32_t* size,
-                                  uint32_t* first, int32_t* status, uint32_t* ioff, uint32_t* nnodes, const uint32_t* list,
-                                  const GgrList* list_h, uint32_t* pending, GgrList* pending_h, int sm_count, int32_t* method,
-                                  uint32_t* id_span, int32_t final_status) {
-  const bool env = method != nullptr;
+void ggr_launch_encode_coop_parse(const GgrLaunch& L, const GgrEncodeView& v, int tier, GgrWork in, GgrWork left, int32_t final_status) {
+  const bool env = v.method != nullptr;
   if (tier == 0) {
     // 4 resident blocks per SM (shared memory)
-    const unsigned nb = ggr_persistent_grid(n, CE_WARPS, sm_count, 4);
-    if (env) ce_launch<CoopEnc, true, true>(st, nb, n, blob, n_msgs, msg_id, in, in_off, ir, size, first, status, ioff, nnodes, list, list_h, pending, pending_h, method, id_span, final_status);
-    else ce_launch<CoopEnc, false, true>(st, nb, n, blob, n_msgs, msg_id, in, in_off, ir, size, first, status, ioff, nnodes, list, list_h, pending, pending_h, method, id_span, final_status);
+    const unsigned nb = ggr_persistent_grid(v.n, CE_WARPS, L.sm_count, 4);
+    if (env) ce_launch<CoopEnc, true, true>(L, nb, v, in, left, final_status);
+    else ce_launch<CoopEnc, false, true>(L, nb, v, in, left, final_status);
   } else {
     // the list length lives on the device: two blocks per SM (shared memory), warps stride over the list
-    const unsigned nb = (unsigned)sm_count * 2u;
-    if (env) ce_launch<CoopEncBig, true, false>(st, nb, n, blob, n_msgs, msg_id, in, in_off, ir, size, first, status, ioff, nnodes, list, list_h, pending, pending_h, method, id_span, final_status);
-    else ce_launch<CoopEncBig, false, false>(st, nb, n, blob, n_msgs, msg_id, in, in_off, ir, size, first, status, ioff, nnodes, list, list_h, pending, pending_h, method, id_span, final_status);
+    const unsigned nb = (unsigned)L.sm_count * 2u;
+    if (env) ce_launch<CoopEncBig, true, false>(L, nb, v, in, left, final_status);
+    else ce_launch<CoopEncBig, false, false>(L, nb, v, in, left, final_status);
   }
 }
 
-void ggr_launch_encode_coop_emit(cudaStream_t st, long long n, const uint8_t* in, const uint64_t* in_off, const uint8_t* ir,
-                                 const uint32_t* ioff, const uint32_t* nnodes, const uint32_t* size, const int32_t* status,
-                                 uint8_t* out, const uint64_t* out_off, int sm_count, const uint32_t* list,
-                                 const GgrList* list_h, uint32_t frame) {
+void ggr_launch_encode_coop_emit(const GgrLaunch& L, const GgrEncodeView& v, GgrWork in, uint8_t* out, const uint64_t* out_off, uint32_t frame) {
   // resident blocks per SM: what the staging buffers in shared memory (and the registers) allow
   static const int resident = ggr_resident_blocks((const void*)k_encode_coop_emit, CE_WARPS * 32, sizeof(CoopEmit) * CE_WARPS, 6);
-  k_encode_coop_emit<<<ggr_persistent_grid(n, CE_WARPS, sm_count, resident), CE_WARPS * 32, sizeof(CoopEmit) * CE_WARPS, st>>>(
-      n, in, (const u64*)in_off, ir, ioff, nnodes, size, status, out, (const u64*)out_off, list, list_h, frame);
+  ggr_enqueue(L, k_encode_coop_emit, ggr_persistent_grid(v.n, CE_WARPS, L.sm_count, resident), CE_WARPS * 32, sizeof(CoopEmit) * CE_WARPS,
+              v.n, v.in, v.in_off, v.ir, v.ioff, v.nnodes, v.size, v.status, out, out_off, in.item, in.h, frame);
 }

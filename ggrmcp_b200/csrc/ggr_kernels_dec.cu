@@ -129,19 +129,13 @@ k_decode_write(const u8* __restrict__ blob, long long n, const i32* __restrict__
   }
 }
 
-void ggr_launch_decode_size(cudaStream_t st, unsigned nb, const uint8_t* blob, long long n, uint32_t n_msgs, const int32_t* msg_id,
-                            const uint8_t* in, const uint64_t* in_off, uint32_t flags, uint32_t* size, uint32_t* mode,
-                            int32_t* status, uint64_t* block_sums, int after_coop, void* sort_pool, uint32_t sort_cap,
-                            const uint32_t* list, const uint32_t* list_n) {
-  k_decode_size<<<nb, GGR_BLOCK, 0, st>>>(blob, n, n_msgs, msg_id, in, (const u64*)in_off, flags, size, mode, status, (u64*)block_sums, after_coop,
-                                          (U4*)sort_pool, sort_cap, list, list_n);
+void ggr_launch_decode_size(const GgrLaunch& L, const GgrDecodeView& v, unsigned nb, int after_coop, const uint32_t* list, const uint32_t* list_n) {
+  ggr_enqueue(L, k_decode_size, nb, GGR_BLOCK, 0, v.blob, v.n, v.n_msgs, v.msg_id, v.in, v.in_off, v.flags, v.size, v.mode, v.status, v.sums,
+              after_coop, (U4*)v.sort_pool, v.sort_cap, list, list_n);
 }
-void ggr_launch_decode_write(cudaStream_t st, unsigned nb, const uint8_t* blob, long long n, const int32_t* msg_id,
-                             const uint8_t* in, const uint64_t* in_off, uint32_t flags, const uint32_t* size,
-                             const uint32_t* mode, int32_t* status, const uint64_t* block_prefix, uint8_t* out,
-                             uint64_t out_cap, uint64_t* out_off, void* sort_pool, uint32_t sort_cap, const uint32_t* list,
-                             const uint32_t* list_n) {
-  k_decode_write<<<nb, GGR_BLOCK, 0, st>>>(blob, n, msg_id, in, (const u64*)in_off, flags, size, mode, status, (const u64*)block_prefix, out, (u64)out_cap, (u64*)out_off,
-                                           (U4*)sort_pool, sort_cap, list, list_n);
+void ggr_launch_decode_write(const GgrLaunch& L, const GgrDecodeView& v, unsigned nb, uint8_t* out, uint64_t out_cap, uint64_t* out_off,
+                             const uint32_t* list, const uint32_t* list_n) {
+  ggr_enqueue(L, k_decode_write, nb, GGR_BLOCK, 0, v.blob, v.n, v.msg_id, v.in, v.in_off, v.flags, v.size, v.mode, v.status, v.sums, out,
+              out_cap, out_off, (U4*)v.sort_pool, v.sort_cap, list, list_n);
 }
 int ggr_decode_max_rec() { return GGR_DEC_MAX_REC; }

@@ -66,21 +66,15 @@ k_diag_write(const u8* __restrict__ in, const u64* __restrict__ in_off, const i3
   }
 }
 
-void ggr_launch_diag_list(cudaStream_t st, long long n, const int32_t* status, uint32_t* list, GgrList* list_h, uint32_t* err_pos,
-                          uint32_t* err_len, uint32_t* text_len) {
-  k_diag_list<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(n, status, list, list_h, err_pos, err_len, text_len);
+void ggr_launch_diag_list(const GgrLaunch& L, long long n, const int32_t* status, GgrWork failing, const GgrDiagView& d) {
+  ggr_enqueue(L, k_diag_list, (unsigned)((n + 255) / 256), 256, 0, n, status, failing.item, failing.h, d.err_pos, d.err_len, d.text_len);
 }
-void ggr_launch_diag_locate(cudaStream_t st, long long n, const uint8_t* in, const uint64_t* in_off, const int32_t* parse_status,
-                            const uint32_t* parse_pos, const uint32_t* list, const GgrList* list_h, uint32_t* err_pos, uint32_t* err_len,
-                            uint32_t* text_len, uint32_t* line, uint32_t* col, int sm_count) {
-  k_diag_locate<<<ggr_persistent_grid(n, DIAG_WARPS, sm_count, 8), DIAG_WARPS * 32, 0, st>>>(in, (const u64*)in_off, parse_status, parse_pos, list,
-                                                                                             list_h, err_pos, err_len, text_len, line, col);
+void ggr_launch_diag_locate(const GgrLaunch& L, const GgrEncodeView& v, GgrWork failing, const GgrDiagView& d) {
+  ggr_enqueue(L, k_diag_locate, ggr_persistent_grid(v.n, DIAG_WARPS, L.sm_count, 8), DIAG_WARPS * 32, 0, v.in, v.in_off, d.parse_status,
+              d.parse_pos, failing.item, failing.h, d.err_pos, d.err_len, d.text_len, d.line, d.col);
 }
-void ggr_launch_diag_write(cudaStream_t st, long long n, const uint8_t* in, const uint64_t* in_off, const int32_t* parse_status,
-                           const uint32_t* list, const GgrList* list_h, const uint32_t* err_pos, const uint32_t* err_len,
-                           const uint32_t* text_len, const uint32_t* line, const uint32_t* col, uint8_t* text, uint64_t text_cap,
-                           const uint64_t* text_off, int sm_count) {
-  k_diag_write<<<ggr_persistent_grid(n, DIAG_WARPS, sm_count, 8), DIAG_WARPS * 32, 0, st>>>(in, (const u64*)in_off, parse_status, list, list_h,
-                                                                                            err_pos, err_len, text_len, line, col, text,
-                                                                                            (u64)text_cap, (const u64*)text_off);
+void ggr_launch_diag_write(const GgrLaunch& L, const GgrEncodeView& v, GgrWork failing, const GgrDiagView& d, uint8_t* text, uint64_t text_cap,
+                           const uint64_t* text_off) {
+  ggr_enqueue(L, k_diag_write, ggr_persistent_grid(v.n, DIAG_WARPS, L.sm_count, 8), DIAG_WARPS * 32, 0, v.in, v.in_off, d.parse_status,
+              failing.item, failing.h, d.err_pos, d.err_len, d.text_len, d.line, d.col, text, text_cap, text_off);
 }

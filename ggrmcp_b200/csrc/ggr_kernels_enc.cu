@@ -122,21 +122,20 @@ k_encode_emit(long long n, const u8* __restrict__ in, const u64* __restrict__ in
   }
 }
 
-void ggr_launch_encode_parse(cudaStream_t st, unsigned nb, const uint8_t* blob, long long n, uint32_t n_msgs, const int32_t* msg_id,
-                             const uint8_t* in, const uint64_t* in_off, uint8_t* ir, uint32_t* size, uint32_t* first,
-                             int32_t* status, uint64_t* block_sums, const uint32_t* list, const uint32_t* list_n, uint32_t* err_pos) {
-  k_encode_parse<<<nb, GGR_BLOCK, 0, st>>>(blob, n, n_msgs, msg_id, in, (const u64*)in_off, ir, size, first, status, (u64*)block_sums,
-                                           list, list_n, err_pos);
+void ggr_launch_encode_parse(const GgrLaunch& L, const GgrEncodeView& v, unsigned nb, const uint32_t* list, const uint32_t* list_n,
+                             uint32_t* err_pos) {
+  ggr_enqueue(L, k_encode_parse, nb, GGR_BLOCK, 0, v.blob, v.n, v.n_msgs, v.msg_id, v.in, v.in_off, v.ir, v.size, v.first, v.status, v.sums,
+              list, list_n, err_pos);
 }
-void ggr_launch_block_sums(cudaStream_t st, unsigned nb, long long n, const uint32_t* size, uint64_t* block_sums) {
-  k_block_sums<<<nb, GGR_BLOCK, 0, st>>>(n, size, (u64*)block_sums);
+void ggr_launch_block_sums(const GgrLaunch& L, unsigned nb, long long n, const uint32_t* size, uint64_t* block_sums) {
+  ggr_enqueue(L, k_block_sums, nb, GGR_BLOCK, 0, n, size, block_sums);
 }
-void ggr_launch_encode_emit(cudaStream_t st, unsigned nb, long long n, const uint8_t* in, const uint64_t* in_off, const uint8_t* ir,
-                            const uint32_t* size, const uint32_t* first, int32_t* status, const uint64_t* block_prefix,
-                            uint8_t* out, uint64_t out_cap, uint64_t* out_off, const uint32_t* skip, uint32_t frame) {
-  k_encode_emit<<<nb, GGR_BLOCK, 0, st>>>(n, in, (const u64*)in_off, ir, size, first, status, (const u64*)block_prefix, out, (u64)out_cap, (u64*)out_off, skip, frame);
+void ggr_launch_encode_emit(const GgrLaunch& L, const GgrEncodeView& v, unsigned nb, uint8_t* out, uint64_t out_cap, uint64_t* out_off,
+                            const uint32_t* skip, uint32_t frame) {
+  ggr_enqueue(L, k_encode_emit, nb, GGR_BLOCK, 0, v.n, v.in, v.in_off, v.ir, v.size, v.first, v.status, v.sums, out, out_cap, out_off, skip,
+              frame);
 }
-void ggr_launch_frame_sizes(cudaStream_t st, long long n, uint32_t* size, const int32_t* status) {
-  k_frame_sizes<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(n, size, status);
+void ggr_launch_frame_sizes(const GgrLaunch& L, const GgrEncodeView& v) {
+  ggr_enqueue(L, k_frame_sizes, (unsigned)((v.n + 255) / 256), 256, 0, v.n, v.size, v.status);
 }
 const void* ggr_kernel_encode_parse() { return (const void*)k_encode_parse; }

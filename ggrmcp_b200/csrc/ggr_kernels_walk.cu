@@ -121,37 +121,31 @@ int ggr_encode_walk_init() {
              : -1;
 }
 
-void ggr_launch_encode_tok2(cudaStream_t st, long long n, const uint8_t* in, const uint64_t* in_off, uint8_t* ir, const uint32_t* list,
-                            const GgrList* list_h, int sm_count) {
+void ggr_launch_encode_tok2(const GgrLaunch& L, const GgrEncodeView& v, GgrWork in) {
   static const int resident = ggr_resident_blocks((const void*)k_encode_tok3, CW_WARPS * 32, 0, 1);
-  k_encode_tok3<<<ggr_persistent_grid(n, CW_WARPS, sm_count, resident), CW_WARPS * 32, 0, st>>>(in, (const u64*)in_off, ir, list, list_h);
+  ggr_enqueue(L, k_encode_tok3, ggr_persistent_grid(v.n, CW_WARPS, L.sm_count, resident), CW_WARPS * 32, 0, v.in, v.in_off, v.ir, in.item, in.h);
 }
 
-void ggr_launch_encode_place(cudaStream_t st, long long n, const uint64_t* in_off, uint8_t* ir, const uint32_t* list, const GgrList* list_h,
-                             int sm_count) {
+void ggr_launch_encode_place(const GgrLaunch& L, const GgrEncodeView& v, GgrWork in) {
   static const int resident = ggr_resident_blocks((const void*)k_encode_place, CW_WARPS * 32, 0, 1);
-  k_encode_place<<<ggr_persistent_grid(n, CW_WARPS, sm_count, resident), CW_WARPS * 32, 0, st>>>((const u64*)in_off, ir, list, list_h);
+  ggr_enqueue(L, k_encode_place, ggr_persistent_grid(v.n, CW_WARPS, L.sm_count, resident), CW_WARPS * 32, 0, v.in_off, v.ir, in.item, in.h);
 }
 
-// tier 0: the listed items; tier 1: what tier 0 left (list / list_h = its pending list; the length lives on the device)
-void ggr_launch_encode_type(cudaStream_t st, int tier, long long n, const uint8_t* blob, uint32_t n_msgs, const int32_t* msg_id, const uint8_t* in,
-                            const uint64_t* in_off, uint8_t* ir, uint32_t* size, uint32_t* first, int32_t* status, uint32_t* ioff,
-                            uint32_t* nnodes, const uint32_t* list, const GgrList* list_h, uint32_t* pending, GgrList* pending_h,
-                            int sm_count) {
+void ggr_launch_encode_type(const GgrLaunch& L, const GgrEncodeView& v, int tier, GgrWork in, GgrWork left) {
   if (tier == 0) {
     const size_t smem = sizeof(CoopWalk) * CW_WARPS;
     static const int resident = ggr_resident_blocks((const void*)k_encode_type<CoopWalk, false, CW_WARPS>, CW_WARPS * 32, smem, 1);
-    k_encode_type<CoopWalk, false, CW_WARPS><<<ggr_persistent_grid(n, CW_WARPS, sm_count, resident), CW_WARPS * 32, smem, st>>>(
-        blob, n_msgs, msg_id, in, (const u64*)in_off, ir, size, first, status, ioff, nnodes, list, list_h, pending, pending_h);
+    ggr_enqueue(L, k_encode_type<CoopWalk, false, CW_WARPS>, ggr_persistent_grid(v.n, CW_WARPS, L.sm_count, resident), CW_WARPS * 32, smem,
+                v.blob, v.n_msgs, v.msg_id, v.in, v.in_off, v.ir, v.size, v.first, v.status, v.ioff, v.nnodes, in.item, in.h, left.item, left.h);
   } else if (tier == 2) {
     // third tier: one warp per SM over what the second left
-    k_encode_type<CoopWalkHuge, true, 1><<<(unsigned)sm_count, 32, sizeof(CoopWalkHuge), st>>>(
-        blob, n_msgs, msg_id, in, (const u64*)in_off, ir, size, first, status, ioff, nnodes, list, list_h, pending, pending_h);
+    ggr_enqueue(L, k_encode_type<CoopWalkHuge, true, 1>, (unsigned)L.sm_count, 32, sizeof(CoopWalkHuge), v.blob, v.n_msgs, v.msg_id, v.in,
+                v.in_off, v.ir, v.size, v.first, v.status, v.ioff, v.nnodes, in.item, in.h, left.item, left.h);
   } else {
     // the list length lives on the device: every resident block
     const size_t smem = sizeof(CoopWalkBig) * CW_WARPS;
     static const int resident = ggr_resident_blocks((const void*)k_encode_type<CoopWalkBig, true, CW_WARPS>, CW_WARPS * 32, smem, 1);
-    k_encode_type<CoopWalkBig, true, CW_WARPS><<<(unsigned)(sm_count * resident), CW_WARPS * 32, smem, st>>>(
-        blob, n_msgs, msg_id, in, (const u64*)in_off, ir, size, first, status, ioff, nnodes, list, list_h, pending, pending_h);
+    ggr_enqueue(L, k_encode_type<CoopWalkBig, true, CW_WARPS>, (unsigned)(L.sm_count * resident), CW_WARPS * 32, smem, v.blob, v.n_msgs,
+                v.msg_id, v.in, v.in_off, v.ir, v.size, v.first, v.status, v.ioff, v.nnodes, in.item, in.h, left.item, left.h);
   }
 }

@@ -48,17 +48,16 @@ k_wrap_write(long long n, const u8* __restrict__ text, const u64* __restrict__ t
   }
 }
 
-void ggr_launch_wrap_size(cudaStream_t st, long long n, const uint8_t* text, const uint64_t* text_off, const int32_t* status,
-                          const uint64_t* ids_off, uint32_t* size, int sm_count) {
-  k_wrap_size<<<ggr_persistent_grid(n, WRAP_WARPS, sm_count, 8), WRAP_WARPS * 32, 0, st>>>(n, text, (const u64*)text_off, status, (const u64*)ids_off, size);
+void ggr_launch_wrap_size(const GgrLaunch& L, long long n, const uint8_t* text, const uint64_t* text_off, const int32_t* status,
+                          const uint64_t* ids_off, uint32_t* size) {
+  ggr_enqueue(L, k_wrap_size, ggr_persistent_grid(n, WRAP_WARPS, L.sm_count, 8), WRAP_WARPS * 32, 0, n, text, text_off, status, ids_off, size);
 }
-void ggr_launch_offsets(cudaStream_t st, unsigned nb, long long n, const uint32_t* size, const uint64_t* block_prefix,
-                        uint64_t* out_off) {
-  k_offsets<<<nb, GGR_BLOCK, 0, st>>>(n, size, (const u64*)block_prefix, (u64*)out_off);
+void ggr_launch_offsets(const GgrLaunch& L, unsigned nb, long long n, const uint32_t* size, const uint64_t* block_prefix, uint64_t* out_off) {
+  ggr_enqueue(L, k_offsets, nb, GGR_BLOCK, 0, n, size, block_prefix, out_off);
 }
-void ggr_launch_wrap_write(cudaStream_t st, long long n, const uint8_t* text, const uint64_t* text_off, int32_t* status,
+void ggr_launch_wrap_write(const GgrLaunch& L, long long n, const uint8_t* text, const uint64_t* text_off, int32_t* status,
                            const uint8_t* ids, const uint64_t* ids_off, const uint32_t* size, uint8_t* out, uint64_t out_cap,
-                           const uint64_t* out_off, int sm_count) {
-  k_wrap_write<<<ggr_persistent_grid(n, WRAP_WARPS, sm_count, 8), WRAP_WARPS * 32, 0, st>>>(n, text, (const u64*)text_off, status, ids, (const u64*)ids_off, size,
-                                                                  out, (u64)out_cap, (const u64*)out_off);
+                           const uint64_t* out_off) {
+  ggr_enqueue(L, k_wrap_write, ggr_persistent_grid(n, WRAP_WARPS, L.sm_count, 8), WRAP_WARPS * 32, 0, n, text, text_off, status, ids, ids_off,
+              size, out, out_cap, out_off);
 }
