@@ -7,6 +7,7 @@ import random
 import pytest
 
 import cases
+from strref import html_string as _go_json_string
 
 
 @pytest.mark.parametrize("name,js,wire", cases.K_REQUESTS)
@@ -336,22 +337,6 @@ def test_coop_decode_large_leaves(hsim):
 
 
 # ---- MCP result wrapping (ggr_wrap.cuh) on 32 fibers ---------------------------------------------
-def _go_json_string(t):
-    """encoding/json appendString, escapeHTML = true, for valid UTF-8"""
-    out = bytearray(b'"')
-    for ch in t.decode("utf-8"):
-        c = ord(ch)
-        if ch in '"\\':
-            out += b"\\" + ch.encode()
-        elif ch in "\n\r\t\b\f":
-            out += {"\n": b"\\n", "\r": b"\\r", "\t": b"\\t", "\b": b"\\b", "\f": b"\\f"}[ch]
-        elif c < 0x20 or ch in "<>&" or c in (0x2028, 0x2029):
-            out += b"\\u%04x" % c
-        else:
-            out += ch.encode("utf-8")
-    return bytes(out + b'"')
-
-
 def test_wrap_result_bodies(oracle):
     import hostsim
     rng = random.Random(4)
