@@ -857,3 +857,78 @@ GGR_DEV int coop_write_item(CoopStage& E, const DecCtx& cx, const U4* tab, u32 n
   }
   return E.bad ? GST_INTERNAL : GST_OK;
 }
+
+// ---- item edge of the reply lock-step kernels (the host simulation calls the same functions) ------------------------
+// Saved entry tables: the first tier's in fixed slots, COOP_TAB_U4 16-byte words per item; the second tier's in the pool,
+// after its header (32 bytes, the bump counter in the first word), at the entry tab_off[item] hands out; nent[item] then
+// has COOP_POOLED set.
+#define COOP_TAB_U4 (2 * GGR_COOP_TAB_ENTRIES)
+#define COOP_POOLED 0x80000000u
+template <class P>
+GGR_DEV P* coop_pool_table(P* pool, u32 toff) {
+  return pool + 2 + 2 * (size_t)toff;
+}
+GGR_DEV const U4* coop_saved_table(const U4* tab, const U4* pool, const u32* tab_off, u32 nent_word, long long item) {
+  return (nent_word & COOP_POOLED) ? coop_pool_table(pool, tab_off[item]) : tab + (size_t)item * COOP_TAB_U4;
+}
+
+// k_decode_coop_size: true when the item was sized and its entry table saved (*ne entries; POOLED, the second tier: in
+// the pool from entry *toff).  A framed item (GGR_DF_GRPC_FRAME) with a bad header is left to the per-thread kernel,
+// which reports it.  Sets cx.in to the item's first 16-byte chunk.
+template <class SH, bool POOLED>
+GGR_DEV bool coop_size_step(SH& S, DecCtx& cx, u32 n_msgs, const i32* msg_id, const u8* in, const u64* in_off, long long item, U4* tab,
+                            U4* pool, u32 pool_cap, u32* ne, u32* sz, u32* toff) {
+  u64 a = in_off[item];
+  const u64 b = in_off[item + 1];
+  const i32 m = msg_id[item];
+  bool framed_ok = true;
+  if (cx.flags & GGR_DF_GRPC_FRAME) {
+    framed_ok = b >= a && ggr_frame_check(in, a, b) == GST_OK;
+    a += GGR_FRAME_BYTES;
+  }
+  bool ok = false;
+  if (framed_ok && m >= 0 && (u32)m < n_msgs && b >= a && b - a <= (u64)GGR_REP_ITEM_MAX) {
+    cx.in = in + (a & ~15ull);
+    const u32 s0 = (u32)(a & 15ull);
+    // one instance of the item code per kernel (both would double the hot instruction stream of the first tier)
+    if (POOLED)
+      ok = coop_size_item(S, cx, (u32)m, s0, s0 + (u32)(b - a), nullptr, ne, sz, coop_pool_table(pool, 0), reinterpret_cast<u32*>(pool),
+                          pool_cap, toff);
+    else
+      ok = coop_size_item(S, cx, (u32)m, s0, s0 + (u32)(b - a), tab + (size_t)item * COOP_TAB_U4, ne, sz);
+  }
+  return ok;
+}
+
+// Lane 0: a sized item's size, mode, status and table; one not sized gets mode PENDING and goes to `left` (if any).
+template <bool POOLED>
+GGR_DEV void coop_size_publish(bool ok, long long item, u32 sz, u32 ne, u32 toff, u32* size, u32* mode, i32* status, u32* nent,
+                               u32* tab_off, GgrWork left) {
+  if (wp_lane() != 0) return;
+  if (ok) {
+    size[item] = sz;
+    mode[item] = GGR_MODE_COOP;
+    status[item] = GST_OK;
+    nent[item] = POOLED ? (ne | COOP_POOLED) : ne;
+    if (POOLED) tab_off[item] = toff;
+  } else {
+    mode[item] = GGR_MODE_PENDING;
+    nent[item] = 0;
+    if (left.item) left.item[ggr_atomic_add_u32(&left.h->n, 1u)] = (u32)item;
+  }
+}
+
+// k_decode_coop_write: the text of an item the size pass took, from its saved table; GST_OK for the others.
+GGR_DEV int coop_write_step(CoopStage& E, DecCtx& cx, const u8* in, const u64* in_off, const u32* size, const u32* mode, const i32* status,
+                            const U4* tab, const u32* nent, const U4* pool, const u32* tab_off, u8* out, const u64* out_off, long long item) {
+  if (mode[item] != GGR_MODE_COOP || status[item] != GST_OK) return GST_OK;
+  const u64 a = in_off[item] + ((cx.flags & GGR_DF_GRPC_FRAME) ? GGR_FRAME_BYTES : 0u);
+  cx.in = in + (a & ~15ull);
+  const u32 nw = nent[item];
+  return coop_write_item(E, cx, coop_saved_table(tab, pool, tab_off, nw, item), nw & ~COOP_POOLED, out + out_off[item], size[item]);
+}
+
+// Lane 0: an item the write pass could not write gets GST_INTERNAL.
+GGR_DEV void coop_write_publish(int ws, long long item, i32* status) {
+  if (ws != GST_OK && wp_lane() == 0) status[item] = GST_INTERNAL;
+}

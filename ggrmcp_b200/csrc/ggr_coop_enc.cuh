@@ -25,6 +25,7 @@
 
 #define CE_MAX_DEPTH 24
 #define CE_MAX_INPUT 65000u
+static_assert(GGR_REQ_ITEM_MAX + 15u <= CE_MAX_INPUT, "a taken item ends by CE_MAX_INPUT at every offset within its chunk");
 #define CE_NIL 0xFFFFu
 #define NF_SIMPLE 2u /* N_STR with NF_ESC: only two-character escapes (the tokenizer's O(1) sizing) */
 
@@ -1404,4 +1405,89 @@ GGR_DEV void ce_emit_item(CoopEmit& E, const u8* in, u32 end, const u8* ir, cons
       else coop_copy_words(in, E.src[k], d, len);
     }
   }
+}
+
+// ---- item edge of the request lock-step kernels (the host simulation calls the same functions) ----------------------
+// Every request lock-step kernel takes items of at most GGR_REQ_ITEM_MAX bytes.
+GGR_DEV bool ce_admit(u64 a, u64 b) { return b >= a && b - a <= (u64)GGR_REQ_ITEM_MAX; }
+
+// Which tier of the lock-step parser runs over the token index k_encode_coop_tok left in the IR region: the first (small
+// tables); the second tokenizes each item itself.
+template <class SH>
+struct CeTokFirst {
+  static constexpr bool value = false;
+};
+template <>
+struct CeTokFirst<CoopEnc> {
+  static constexpr bool value = true;
+};
+
+// k_encode_coop_tok, item `item` of the batch whose input starts at a0: its token index into its IR region.
+template <class TS>
+GGR_DEV void ce_tok_step(TS& S, const CeLut& lut, const u8* in, const u64* in_off, u64 a0, u8* ir, long long item) {
+  const u64 a = in_off[item], b = in_off[item + 1];
+  if (!ce_admit(a, b)) return;
+  const GgrRegion r = ggr_item_region(a0, a, b, (u64)item);
+  const u32 s0 = (u32)(a & 15ull);
+  ce_tok_item(S, lut, in + (a & ~15ull), s0, s0 + (u32)(b - a), ir + r.node_off * 16, r.cap);
+}
+
+// k_encode_coop_parse: true when the item was parsed into its IR region, *res filled (id_pos from the item's first byte).
+// ENV: the item is a whole request body, its message type comes from the tool name.
+template <class SH, bool ENV, bool PRE>
+GGR_DEV bool ce_parse_step(SH& S, const CeLut& lut, const Tables& T, u32 n_msgs, const i32* msg_id, const u8* in,
+                           const u64* in_off, u64 a0, u8* ir, u32* ioff, long long item, EncResult* res) {
+  const u64 a = in_off[item], b = in_off[item + 1];
+  const i32 m = ENV ? 0 : msg_id[item];
+  if (m < 0 || (u32)m >= n_msgs || !ce_admit(a, b)) return false;
+  const GgrRegion r = ggr_item_region(a0, a, b, (u64)item);
+  const u32 s0 = (u32)(a & 15ull);
+  const bool ok = ce_parse_item<SH, ENV, PRE>(S, lut, T, (u32)m, in + (a & ~15ull), s0, s0 + (u32)(b - a), ir + r.node_off * 16,
+                                              ioff + r.node_off, r.cap, res);
+  if (ENV) res->id_pos -= s0;
+  return ok;
+}
+
+// nnodes of an item the lock-step emitter writes: node count | index of the first node within the item's region << 16.
+GGR_DEV u32 ce_nodes_word(u32 n_nodes, u32 first_node) { return n_nodes | (first_node << 16); }
+
+// Lane 0: a parsed item's size, first node, status and node count (and the body's method and id span), where items of
+// more than CE_STAGE wire bytes get none (the per-thread emitter writes them).  An item not parsed gets final_status
+// when that is >= 0 (the last tier of request bodies: no per-thread path), or goes to `left`.
+template <bool ENV>
+GGR_DEV void ce_parse_publish(bool ok, const EncResult& res, long long item, u32* size, u32* first, i32* status, u32* nnodes,
+                              i32* method, u32* id_span, i32 final_status, GgrWork left) {
+  if (wp_lane() != 0) return;
+  if (ok) {
+    size[item] = res.size;
+    first[item] = res.first;
+    status[item] = GST_OK;
+    nnodes[item] = res.size <= CE_STAGE ? ce_nodes_word(res.n_nodes, 0) : 0;
+    if (ENV) {
+      method[item] = (i32)res.method;
+      id_span[2 * item] = res.id_pos;
+      id_span[2 * item + 1] = res.id_len;
+    }
+  } else {
+    size[item] = 0;
+    nnodes[item] = 0;
+    first[item] = GGR_NIL;
+    if (final_status >= 0) status[item] = final_status;
+    else left.item[ggr_atomic_add_u32(&left.h->n, 1u)] = (u32)item;
+  }
+}
+
+// k_encode_coop_emit: pass B of an item the lock-step parser or the walker took with more than one node, behind the
+// frame-byte message header k_encode_emit wrote.  True when it wrote the item.
+GGR_DEV bool ce_emit_step(CoopEmit& E, const u8* in, const u64* in_off, u64 a0, const u8* ir, const u32* ioff, const u32* nnodes,
+                          const u32* size, const i32* status, u8* out, const u64* out_off, u32 frame, long long item) {
+  const u32 nw = nnodes[item];
+  const u32 nn = nw & 0xFFFFu;
+  const u32 sz = size[item];
+  if (nn <= 1 || sz <= frame || status[item] != GST_OK) return false;
+  const u64 a = in_off[item], b = in_off[item + 1];
+  const u64 node_off = ggr_item_region(a0, a, b, (u64)item).node_off + (u64)(nw >> 16);
+  ce_emit_item(E, in + (a & ~15ull), (u32)(a & 15ull) + (u32)(b - a), ir + node_off * 16, ioff + node_off, nn, out + out_off[item] + frame,
+               sz - frame);
+  return true;
 }

@@ -807,7 +807,7 @@ static int run_encode_kernels(ggr_engine* e, const ggr_schema* s, Scratch& sc, i
     prof.span(P_ENCODE_PARSE);
   } else {
     // router: small (and oversized) items straight to the per-thread parser
-    ggr_enqueue(L, k_route, (unsigned)((n + 255) / 256), 256, 0, n, in_off, e->min_json, 65000u - 16u, W.lockstep.item, &W.lockstep.h->n,
+    ggr_enqueue(L, k_route, (unsigned)((n + 255) / 256), 256, 0, n, in_off, e->min_json, GGR_REQ_ITEM_MAX, W.lockstep.item, &W.lockstep.h->n,
                 W.per_thread.item, &W.per_thread.h->n, nullptr);
     if (e->use_walk) {
       ggr_launch_encode_tok2(L, v, W.lockstep);
@@ -874,7 +874,7 @@ static int run_decode_kernels(ggr_engine* e, const ggr_schema* s, Scratch& sc, i
   const GgrLaunch L{st, e->sm_count, &e->launches};
   const GgrDecodeView v = decode_view(s, sc, n, msg_id, in, in_off, status, flags, sort_cap, pool_cap);
   if (coop) {
-    ggr_enqueue(L, k_route, (unsigned)((n + 255) / 256), 256, 0, n, in_off, e->min_wire, 0x3FFFFF00u, W.lockstep.item, &W.lockstep.h->n,
+    ggr_enqueue(L, k_route, (unsigned)((n + 255) / 256), 256, 0, n, in_off, e->min_wire, GGR_REP_ITEM_MAX, W.lockstep.item, &W.lockstep.h->n,
                 nullptr, nullptr, v.mode);
     ggr_launch_decode_coop_size(L, v, W.lockstep, W.tier1_left);
     prof.span(P_DECODE_COOP_SIZE);
@@ -981,7 +981,7 @@ static int run_request_dev(ggr_engine* e, const ggr_schema* s, Scratch& sc, int6
     v.method = method;
     v.id_span = id_span;
     // bodies above the parser's input limit cannot be taken
-    ggr_enqueue(L, k_route, (unsigned)((n + 255) / 256), 256, 0, n, in_off, 0u, 65000u - 16u, W.lockstep.item, &W.lockstep.h->n, W.rest.item,
+    ggr_enqueue(L, k_route, (unsigned)((n + 255) / 256), 256, 0, n, in_off, 0u, GGR_REQ_ITEM_MAX, W.lockstep.item, &W.lockstep.h->n, W.rest.item,
                 &W.rest.h->n, nullptr);
     ggr_launch_encode_coop_tok(L, v, W.lockstep);
     ggr_launch_encode_coop_parse(L, v, 0, W.lockstep, W.tier1_left);

@@ -21,12 +21,6 @@ inline void ggr_enqueue(const GgrLaunch& L, void (*kernel)(P...), unsigned grid,
   *L.launches += 1;
 }
 
-// A lock-step work list: its header (count and tickets, ggr_layout.h) and its item indices.
-struct GgrWork {
-  GgrList* h;
-  uint32_t* item;
-};
-
 // Either direction: the batch, its items' output sizes and statuses, and sums (one word per block of GGR_BLOCK items).
 struct GgrBatchView {
   const uint8_t* blob;

@@ -22,37 +22,18 @@ k_encode_tok3(const u8* __restrict__ in, const u64* __restrict__ in_off, u8* __r
   if ((threadIdx.x & 31u) == 0) cw_tile_init(&tiles[warp]);
   __syncthreads();
   u32 ph = 0;
-  const long long total = (long long)list_h->n;
   const u64 a0 = in_off[0];
-  u32* ticket = const_cast<u32*>(&list_h->tok_ticket);
-  u32 drawn = wp_ticket_draw(ticket);
-  for (long long slot = wp_ticket_take(drawn); slot < total; slot = wp_ticket_take(drawn)) {
-    drawn = wp_ticket_draw(ticket);
-    const long long item = (long long)list[slot];
-    const u64 a = in_off[item], b = in_off[item + 1];
-    if (b < a || b - a > (u64)CE_MAX_INPUT - 16u) continue;
-    const GgrRegion r = ggr_item_region(a0, a, b, (u64)item);
-    const u32 s0 = (u32)(a & 15ull);
-    cw_tok_item(&tiles[warp], ph, lut, in + (a & ~15ull), s0, s0 + (u32)(b - a), ir + r.node_off * 16, r.cap);
-  }
+  for (WpTickets<1> t(const_cast<u32*>(&list_h->tok_ticket), (long long)list_h->n); t.take();)
+    cw_tok_step(&tiles[warp], ph, lut, in, in_off, a0, ir, (long long)list[t.slot]);
 }
 
 __global__ void __launch_bounds__(CW_WARPS * 32, CW_PLACE_BLOCKS)
 k_encode_place(const u64* __restrict__ in_off, u8* __restrict__ ir, const u32* __restrict__ list, const GgrList* __restrict__ list_h) {
   __shared__ CwPlaceSh S[CW_WARPS];
   const u32 warp = threadIdx.x >> 5;
-  const long long total = (long long)list_h->n;
   const u64 a0 = in_off[0];
-  u32* ticket = const_cast<u32*>(&list_h->place_ticket);
-  u32 drawn = wp_ticket_draw(ticket);
-  for (long long slot = wp_ticket_take(drawn); slot < total; slot = wp_ticket_take(drawn)) {
-    drawn = wp_ticket_draw(ticket);
-    const long long item = (long long)list[slot];
-    const u64 a = in_off[item], b = in_off[item + 1];
-    if (b <= a || b - a > (u64)CE_MAX_INPUT - 16u) continue;
-    const GgrRegion r = ggr_item_region(a0, a, b, (u64)item);
-    cw_place_item(S[warp], ir + r.node_off * 16, r.cap, CoopWalkHuge::MAX_NODE);
-  }
+  for (WpTickets<1> t(const_cast<u32*>(&list_h->place_ticket), (long long)list_h->n); t.take();)
+    cw_place_step(S[warp], in_off, a0, ir, (long long)list[t.slot]);
 }
 
 // Every item the walker handles gets size / status / node count written here; the others are appended to
@@ -69,47 +50,17 @@ k_encode_type(const u8* __restrict__ blob, u32 n_msgs, const i32* __restrict__ m
               const GgrList* __restrict__ list_h, u32* __restrict__ pending, GgrList* __restrict__ pending_h) {
   extern __shared__ __align__(16) unsigned char smem[];
   SH* S = reinterpret_cast<SH*>(smem);
-  const u32 warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const long long total = (long long)list_h->n;
+  const u32 warp = threadIdx.x >> 5;
   const Tables T = ggr_tables(blob);
   const u64 a0 = in_off[0];
-  u32* ticket = const_cast<u32*>(&list_h->item_ticket);
   // two tickets in flight (the draw's latency stays off the path).  A bulk L2 prefetch of the next item's index, records
   // and text (cp.async.bulk.prefetch.L2) cost more than it saved here when tuned before the H100 port: the index was written by the two kernels in
   // front of this one and is L2-resident already
-  u32 drawn = wp_ticket_draw(ticket);
-  long long slot = wp_ticket_take(drawn);
-  drawn = wp_ticket_draw(ticket);
-  while (slot < total) {
-    const long long next = wp_ticket_take(drawn);
-    drawn = wp_ticket_draw(ticket);
-    const long long item = (long long)list[slot];
-    const u64 a = in_off[item], b = in_off[item + 1];
-    const i32 m = msg_id[item];
-    bool ok = false;
+  for (WpTickets<2> t(const_cast<u32*>(&list_h->item_ticket), (long long)list_h->n); t.take();) {
+    const long long item = (long long)list[t.slot];
     EncResult res;
-    res.size = 0;
-    res.n_nodes = 0;
-    res.method = 0;
-    if (m >= 0 && (u32)m < n_msgs && b >= a && b - a <= (u64)CE_MAX_INPUT - 16u) {
-      const GgrRegion r = ggr_item_region(a0, a, b, (u64)item);
-      const u32 s0 = (u32)(a & 15ull);
-      ok = cw_type_item<SH, FULL>(S[warp], T, (u32)m, in + (a & ~15ull), s0, s0 + (u32)(b - a), ir + r.node_off * 16, ioff + r.node_off, r.cap, &res);
-    }
-    if (lane == 0) {
-      if (ok) {
-        size[item] = res.size;
-        first[item] = GGR_NIL;
-        status[item] = GST_OK;
-        nnodes[item] = res.n_nodes | (res.method << 16);  // node count | where the nodes start within the region
-      } else {
-        size[item] = 0;
-        nnodes[item] = 0;
-        first[item] = GGR_NIL;
-        pending[atomicAdd(&pending_h->n, 1u)] = (u32)item;
-      }
-    }
-    slot = next;
+    const bool ok = cw_type_step<SH, FULL>(S[warp], T, n_msgs, msg_id, in, in_off, a0, ir, ioff, item, &res);
+    cw_type_publish(ok, res, item, size, first, status, nnodes, GgrWork{pending_h, pending});
   }
 }
 

@@ -1,5 +1,6 @@
 // ggr_layout.h - the scratch layout of a batch that the engine, the kernels and the host simulation share: where each
-// item's IR region lies, how large the IR and its output offsets are, and the header of a lock-step work list.
+// item's IR region lies, how large the IR and its output offsets are, the largest items the lock-step kernels take, and
+// the lock-step work lists.
 // Plain C++ with no CUDA dependencies, so the host simulation (tests/hostsim) includes it as well.
 #pragma once
 #include <stddef.h>
@@ -39,3 +40,14 @@ struct GgrList {
   uint32_t item_ticket;   // k_encode_type, k_encode_coop_parse and the reply write kernel
   uint32_t place_ticket;  // k_encode_place
 };
+// A lock-step work list: its header and its item indices.
+struct GgrWork {
+  GgrList* h;
+  uint32_t* item;
+};
+
+// The largest items (in input bytes) the lock-step kernels take; longer ones go to the per-thread kernels.  Request side:
+// positions within an item's first 16-byte chunk are 16 bits wide, so an item that starts at any offset of its chunk must
+// end by byte CE_MAX_INPUT (ggr_coop_enc.cuh).  Reply side: below 2^30 bytes, the lengths the writer's hand-off list keeps.
+#define GGR_REQ_ITEM_MAX 64984u
+#define GGR_REP_ITEM_MAX 0x3FFFFF00u

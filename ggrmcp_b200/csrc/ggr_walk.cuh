@@ -1406,3 +1406,58 @@ GGR_DEV bool cw_type_item(SH& S, const Tables& T, u32 root_msg, const u8* in, u3
   res->method = shift;  // where the IR nodes of this item start within its region (in nodes): travels with n_nodes
   return true;
 }
+
+// ---- item edge of the walker's kernels (the host simulation calls the same functions) ----------------------------------
+// Admission is ce_admit's.  An empty item has no token index and no value records: k_encode_tok3 and k_encode_place skip
+// it (cw_indexed), k_encode_type takes it as an empty message (cw_type_item).
+GGR_DEV bool cw_indexed(u64 a, u64 b) { return b != a && ce_admit(a, b); }
+
+// k_encode_tok3, item `item` of the batch whose input starts at a0.  tl / ph: as cw_tok_item.
+GGR_DEV void cw_tok_step(CwTile* tl, u32& ph, const CwLut& lut, const u8* in, const u64* in_off, u64 a0, u8* ir, long long item) {
+  const u64 a = in_off[item], b = in_off[item + 1];
+  if (!cw_indexed(a, b)) return;
+  const GgrRegion r = ggr_item_region(a0, a, b, (u64)item);
+  const u32 s0 = (u32)(a & 15ull);
+  cw_tok_item(tl, ph, lut, in + (a & ~15ull), s0, s0 + (u32)(b - a), ir + r.node_off * 16, r.cap);
+}
+
+// k_encode_place
+GGR_DEV void cw_place_step(CwPlaceSh& S, const u64* in_off, u64 a0, u8* ir, long long item) {
+  const u64 a = in_off[item], b = in_off[item + 1];
+  if (!cw_indexed(a, b)) return;
+  const GgrRegion r = ggr_item_region(a0, a, b, (u64)item);
+  cw_place_item(S, ir + r.node_off * 16, r.cap, CoopWalkHuge::MAX_NODE);
+}
+
+// k_encode_type: true when the item was taken (IR nodes and their offsets written, *res filled).
+template <class SH, bool FULL>
+GGR_DEV bool cw_type_step(SH& S, const Tables& T, u32 n_msgs, const i32* msg_id, const u8* in, const u64* in_off, u64 a0, u8* ir,
+                          u32* ioff, long long item, EncResult* res) {
+  const u64 a = in_off[item], b = in_off[item + 1];
+  const i32 m = msg_id[item];
+  res->size = 0;
+  res->n_nodes = 0;
+  res->method = 0;
+  if (m < 0 || (u32)m >= n_msgs || !ce_admit(a, b)) return (CW_WHY(1), false);
+  const GgrRegion r = ggr_item_region(a0, a, b, (u64)item);
+  const u32 s0 = (u32)(a & 15ull);
+  return cw_type_item<SH, FULL>(S, T, (u32)m, in + (a & ~15ull), s0, s0 + (u32)(b - a), ir + r.node_off * 16, ioff + r.node_off, r.cap,
+                                res);
+}
+
+// Lane 0: a taken item's size, status and nodes (for k_encode_coop_emit); one not taken goes to `left`.
+GGR_DEV void cw_type_publish(bool ok, const EncResult& res, long long item, u32* size, u32* first, i32* status, u32* nnodes,
+                             GgrWork left) {
+  if (wp_lane() != 0) return;
+  if (ok) {
+    size[item] = res.size;
+    first[item] = GGR_NIL;
+    status[item] = GST_OK;
+    nnodes[item] = ce_nodes_word(res.n_nodes, res.method);  // cw_type_item: method = where the nodes start
+  } else {
+    size[item] = 0;
+    nnodes[item] = 0;
+    first[item] = GGR_NIL;
+    left.item[ggr_atomic_add_u32(&left.h->n, 1u)] = (u32)item;
+  }
+}

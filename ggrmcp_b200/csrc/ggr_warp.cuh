@@ -178,6 +178,31 @@ inline u32 wp_atomic_max(u32* p, u32 v) {
 }
 #endif
 
+// A persistent warp's walk over the slots [0, total) of a work list, drawn from `ticket`:
+//   for (WpTickets<N> t(ticket, total); t.take();) { ... t.slot ... }
+// IN_FLIGHT 1: the draw for the next slot is in flight while the body runs.  IN_FLIGHT 2: the slot after this one is
+// already known (t.next, for an L2 prefetch of that item; >= total: none) and the draw for the one after that is in flight.
+template <int IN_FLIGHT>
+struct WpTickets {
+  u32* ticket;
+  long long total, slot, next;
+  u32 drawn;
+  GGR_DEV WpTickets(u32* ticket_, long long total_) : ticket(ticket_), total(total_) {
+    drawn = wp_ticket_draw(ticket);
+    if (IN_FLIGHT == 2) {
+      next = wp_ticket_take(drawn);
+      drawn = wp_ticket_draw(ticket);
+    }
+  }
+  GGR_DEV bool take() {  // false: the list is done
+    slot = IN_FLIGHT == 2 ? next : wp_ticket_take(drawn);
+    if (slot >= total) return false;
+    if (IN_FLIGHT == 2) next = wp_ticket_take(drawn);
+    drawn = wp_ticket_draw(ticket);
+    return true;
+  }
+};
+
 #define WP_SYNC() wp_sync_(__LINE__)
 #define WP_BALLOT(p) wp_ballot_((p), __LINE__)
 #define WP_SHFL(v, src) wp_shfl_((v), (src), __LINE__)

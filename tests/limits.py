@@ -47,7 +47,8 @@ W5_NODE_PT_LAST = 14        # ... the per-thread parser
 W5_COOP_LAST = 21           # nesting through bench.All.recursive the lock-step parser takes (the walker: field index >= 32)
 W5_PT_LAST = 30             # ... the per-thread parser (GGR_MAX_DEPTH frames, the root included)
 MAX_DEPTH = 32              # GGR_MAX_DEPTH: the per-thread parser answers GGR_ST_DEPTH beyond it
-CE_MAX_INPUT = 65000        # CE_MAX_INPUT: the walker takes items that end at or before this byte
+CE_MAX_INPUT = 65000        # CE_MAX_INPUT: 16-bit positions of the request lock-step kernels
+REQ_ITEM_MAX = 64984        # GGR_REQ_ITEM_MAX: the longest request item the lock-step kernels take
 CE_STAGE_BUF = 4864         # CE_STAGE_BUF: wire bytes assembled in shared memory
 CE_STAGE = 8192             # CE_STAGE: the walker's first tier leaves items with more wire bytes
 CE_LONG_MAX = 32            # CE_LONG_MAX: the emitter's hand-off list
@@ -286,11 +287,11 @@ def request_items(oracle):
     for d in _around(W5_COOP_LAST) + _around(W5_PT_LAST, (40,)):
         add("W5", _side(d, W5_COOP_LAST), _nest(d))
     add("W5", "above", _nest(W5_COOP_LAST + 1)[:-3], True)
-    # W6: 16-bit positions: the walker takes items that end by byte 65000 (start offset included)
+    # W6: 16-bit positions: the lock-step kernels take items of at most 64984 bytes, which end by byte 65000 at any offset
     for n in (64983, 64984, 64985, 64986, 64999, 65000, 65001, 65002, 70000):
         js = _fit(lambda L: _str_item(L, b',"r_int32":[1,2,3],"f_msg":{"x":1,"y":"yy"}'), n, len)
-        add("W6", _side(n, CE_MAX_INPUT), js)
-    js = bytearray(_fit(lambda L: _str_item(L), CE_MAX_INPUT, len))
+        add("W6", _side(n, REQ_ITEM_MAX), js)
+    js = bytearray(_fit(lambda L: _str_item(L), REQ_ITEM_MAX, len))
     js[-4] = 0xFF
     add("W6", "at", bytes(js), True)
     # W7: wire bytes staged (<= 4864) or written in place; the first tier leaves items with more than 8192

@@ -218,8 +218,8 @@ def test_request_limits(oracle, hsim, monkeypatch, row):
         if row == "W6":
             for io in (0, 15):
                 rc, why = _request_parity(oracle, hsim, it, i, io)
-                if not it.damaged:  # positions are 16 bits: the walker takes items that end by byte 65000
-                    assert (rc == 0) == (io + len(it.data) <= LM.CE_MAX_INPUT), (len(it.data), io, rc, why)
+                if not it.damaged:  # positions are 16 bits: the walker takes items of at most 64984 bytes at any offset
+                    assert (rc == 0) == (len(it.data) <= LM.REQ_ITEM_MAX), (len(it.data), io, rc, why)
                     assert rc == 0 or why == 1
             continue
         res[i] = _request_parity(oracle, hsim, it, i)
