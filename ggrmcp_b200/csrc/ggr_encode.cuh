@@ -334,6 +334,26 @@ GGR_DEV int kind_bits(u32 k) {
   return (k == GK_INT32 || k == GK_UINT32 || k == GK_SINT32 || k == GK_FIXED32 || k == GK_SFIXED32) ? 32 : 64;
 }
 
+// Does the decoded text of the valid string token at q end in a character strings.TrimSpace removes?  The ASCII spaces
+// and U+0085, U+00A0, U+1680, U+2000-200A, U+2028, U+2029, U+202F, U+205F, U+3000.  (A quoted number that starts with
+// one fails the number parser.)
+GGR_DEV bool str_ends_in_space(const u8* in, u32 q, u32 end) {
+  StrIter it;
+  it.init(in, q, end);
+  u32 c2 = 0, c1 = 0, c0 = 0;  // the last three decoded bytes, c0 the last
+  while (!it.eof()) {
+    c2 = c1;
+    c1 = c0;
+    c0 = it.peek();
+    it.adv();
+  }
+  if (c0 == ' ' || (c0 - 9u) < 5u) return true;
+  if (c1 == 0xC2u) return c0 == 0x85u || c0 == 0xA0u;
+  if (c2 == 0xE1u) return c1 == 0x9Au && c0 == 0x80u;
+  if (c2 == 0xE2u) return (c1 == 0x80u && (c0 - 0x80u <= 0x0Au || c0 == 0xA8u || c0 == 0xA9u || c0 == 0xAFu)) || (c1 == 0x81u && c0 == 0x9Fu);
+  return c2 == 0xE3u && c1 == 0x80u && c0 == 0x80u;
+}
+
 // Parses one scalar value of `kind` at the reader.  Returns a GST_* status.
 GGR_DEV int parse_scalar(EncCtx& cx, Rd& r, u32 kind, i32 child, Leaf* l) {
   u32 c = r.get();
@@ -356,14 +376,7 @@ GGR_DEV int parse_scalar(EncCtx& cx, Rd& r, u32 kind, i32 child, Leaf* l) {
         StrIter it;
         it.init(cx.in, q, cx.end);
         if (!parse_number(it, &t)) return GST_INVALID_VALUE;
-        // strings.TrimSpace must be a no-op: the last decoded byte may not be ASCII space
-        {
-          StrIter e2;
-          e2.init(cx.in, q, cx.end);
-          u32 last = 0;
-          while (!e2.eof()) { last = e2.peek(); e2.adv(); }
-          if (last == ' ' || (last - 9u) < 5u) return GST_INVALID_VALUE;
-        }
+        if (str_ends_in_space(cx.in, q, cx.end)) return GST_INVALID_VALUE;  // strings.TrimSpace must be a no-op
       } else if (c == '-' || c - '0' < 10u) {
         RawIter it = {&r};
         if (!parse_number(it, &t)) return GST_SYNTAX;
@@ -457,11 +470,7 @@ GGR_DEV int parse_scalar(EncCtx& cx, Rd& r, u32 kind, i32 child, Leaf* l) {
           StrIter it;
           it.init(cx.in, q, cx.end);
           if (!parse_number(it, &t)) return GST_INVALID_VALUE;
-          StrIter e2;
-          e2.init(cx.in, q, cx.end);
-          u32 last = 0;
-          while (!e2.eof()) { last = e2.peek(); e2.adv(); }
-          if (last == ' ' || (last - 9u) < 5u) return GST_INVALID_VALUE;
+          if (str_ends_in_space(cx.in, q, cx.end)) return GST_INVALID_VALUE;  // strings.TrimSpace must be a no-op
           StrIter again;
           again.init(cx.in, q, cx.end);
           ok = float_from_token(again, t, is32, &bits);

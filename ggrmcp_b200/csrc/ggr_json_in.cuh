@@ -313,7 +313,7 @@ GGR_DEV bool parse_number(It& it, NumTok* t) {
       it.adv();
       c = it.get();
     } while (c - '0' < 10u);
-    // beyond 10^8 the exponent stays clamped: an integer kind fails on it below (strconv.Atoi's range error, see oracle),
+    // beyond 10^8 the exponent stays clamped: an integer kind with a nonzero digit fails on it (num_to_int),
     // strconv.ParseFloat goes on - 0.0e2964595747023549 is 0, 1e-99999999999 underflows to 0, 1e99999999999 is out of range
     if (eneg) exp = -exp;
   }
@@ -331,11 +331,13 @@ GGR_DEV bool parse_number(It& it, NumTok* t) {
 // Returns false when the token is not an integer in range [upstream normalizeToIntString +
 // strconv.ParseInt/ParseUint].
 GGR_DEV bool num_to_int(const NumTok& t, bool is_signed, int bits, u64* out) {
-  if (t.exp > 100000000 || t.exp < -100000000) return false;  // strconv.Atoi of the exponent fails (see oracle): no integer, whatever the digits
-  if (t.m == 0 && !t.ovf) {
+  if (t.m == 0 && !t.ovf) {  // no nonzero digit: 0 whatever the exponent (normalizeToIntString returns before reading it)
     *out = 0;
     return true;
   }
+  // beyond 10^8 the exponent is clamped: strconv.ParseInt(exp, 10, 32) fails, or a nonzero value has more than 20 digits
+  // or shifts nonzero digits out
+  if (t.exp > 100000000 || t.exp < -100000000) return false;
   if (t.ovf || t.k < 0 || t.k > 19) return false;
   // upstream's digit-count guard: integer-part digits + exponent may not exceed 20
   if (t.exp >= 0 && (i64)t.int_digits + t.exp > 20) return false;

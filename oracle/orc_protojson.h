@@ -262,6 +262,13 @@ struct PJTokens {
   }
 };
 
+// unicode.IsSpace, what strings.TrimSpace removes: the ASCII set and U+0085, U+00A0, U+1680, U+2000-200A, U+2028/9,
+// U+202F, U+205F, U+3000
+inline bool go_space_rune(uint32_t r) {
+  return r == ' ' || (r >= 9 && r <= 13) || r == 0x85 || r == 0xA0 || r == 0x1680 || (r >= 0x2000 && r <= 0x200A) || r == 0x2028 ||
+         r == 0x2029 || r == 0x202F || r == 0x205F || r == 0x3000;
+}
+
 // ---- number token -> integer (Token.Int / Token.Uint via getIntStr/normalizeToIntString) ----
 struct NumParts {
   bool neg = false;
@@ -292,7 +299,7 @@ inline bool pj_number_parts(const std::string& raw, NumParts& np) {
   if (n - i >= 2 && (raw[i] == 'e' || raw[i] == 'E')) {
     i++;
     std::string ex = raw.substr(i);
-    // strconv.Atoi: optional sign, digits; range error on overflow
+    // the exponent's text: optional sign, digits (read as a 32-bit integer in pj_normalize_int)
     size_t k = 0;
     bool eneg = false;
     if (ex[k] == '+' || ex[k] == '-') {
@@ -303,8 +310,7 @@ inline bool pj_number_parts(const std::string& raw, NumParts& np) {
     long v = 0;
     for (; k < ex.size(); k++) {
       if (ex[k] < '0' || ex[k] > '9') return false;
-      v = v * 10 + (ex[k] - '0');
-      if (v > 100000000L) return false;  // Atoi range error surrogate: such exponents never yield an int
+      if (v <= (1L << 32)) v = v * 10 + (ex[k] - '0');  // clamped: beyond int32 either way
     }
     np.exp = eneg ? -v : v;
     i = n;
@@ -313,10 +319,11 @@ inline bool pj_number_parts(const std::string& raw, NumParts& np) {
 }
 inline bool pj_normalize_int(const NumParts& np, std::string& out) {
   size_t is = np.intp.size(), fs = np.frac.size();
-  if (is == 0 && fs == 0) {
+  if (is == 0 && fs == 0) {  // no nonzero digit: 0 whatever the exponent (upstream returns before it reads the exponent)
     out = "0";
     return true;
   }
+  if (np.exp > INT32_MAX || np.exp < INT32_MIN) return false;  // strconv.ParseInt(exp, 10, 32) fails
   std::string num;
   if (np.exp >= 0) {
     if ((long)fs > np.exp) return false;
@@ -612,13 +619,15 @@ struct PJUnmarshal {
     }
     if (t.kind != K_STRING) return false;
     const Bytes& s = t.str;
-    // strings.TrimSpace must be a no-op
+    // strings.TrimSpace must be a no-op: neither the first nor the last rune is Unicode White_Space (a number token may
+    // end in front of a multi-byte space, so "1\u00a0" is refused here, not by the number parser)
     if (!s.empty()) {
-      auto sp = [](uint8_t c) { return c == ' ' || c == '\t' || c == '\n' || c == '\v' || c == '\f' || c == '\r' || c == 0x85 || c == 0xA0; };
-      // (TrimSpace is Unicode-aware; ASCII + U+0085/U+00A0 cannot be told apart bytewise here,
-      //  multi-byte spaces make the number parser fail anyway)
-      if (sp((uint8_t)s.front()) && (uint8_t)s.front() < 0x80) return false;
-      if (sp((uint8_t)s.back()) && (uint8_t)s.back() < 0x80) return false;
+      int w;
+      if (go_space_rune(utf8_decode((const uint8_t*)s.data(), s.size(), w))) return false;
+      size_t k = s.size() - 1;
+      while (k > 0 && ((uint8_t)s[k] & 0xC0) == 0x80 && s.size() - k < 4) k--;
+      uint32_t r = utf8_decode((const uint8_t*)s.data() + k, s.size() - k, w);
+      if ((size_t)w == s.size() - k && go_space_rune(r)) return false;
     }
     // a fresh decoder reads ONE token from the string; it must be a Number
     Err e2;
@@ -810,14 +819,10 @@ struct PJUnmarshal {
     std::string str(t.str.begin(), t.str.end());
     // strings.TrimSpace: Unicode White_Space (ASCII set + U+0085, U+00A0, U+1680, U+2000-200A, U+2028/9, U+202F, U+205F, U+3000)
     auto space_at = [&](size_t i, size_t& w) -> bool {
-      unsigned char c = (unsigned char)str[i];
-      if (c == ' ' || (c >= 9 && c <= 13)) { w = 1; return true; }
-      if (c < 0x80) return false;
       int ww;
       uint32_t r = utf8_decode((const uint8_t*)str.data() + i, str.size() - i, ww);
       w = (size_t)ww;
-      return r == 0x85 || r == 0xA0 || r == 0x1680 || (r >= 0x2000 && r <= 0x200A) || r == 0x2028 || r == 0x2029 || r == 0x202F ||
-             r == 0x205F || r == 0x3000;
+      return go_space_rune(r);
     };
     size_t b = 0, e = str.size(), w;
     while (b < e && space_at(b, w)) b += w;

@@ -121,11 +121,18 @@ ENCODE_EDGE = [
     (P + "ProcessNodeRequest", b'{"invalid_field":"value"}', "unknown_field"),
     ("google.protobuf.Timestamp", b'"2024-01-01T12:00:00Z"', None), ("google.protobuf.Timestamp", b'{}', None),
     # exponents beyond 10^8 (found by fuzzing): strconv.ParseFloat goes on - a zero mantissa stays 0, a negative exponent
-    # underflows to 0, a positive one is out of range - while an integer kind fails on strconv.Atoi of the exponent
+    # underflows to 0, a positive one is out of range; an integer kind is 0 for a zero mantissa whatever the exponent
+    # (found by the integer reference) and fails on strconv.ParseInt(exp, 10, 32) otherwise
     (A, b'{"f_double":0.0e002964595747023549}', None), (A, b'{"f_double":1e-99999999999,"f_float":-0e99999999999}', None),
     (A, b'{"f_double":1e99999999999}', None), (A, b'{"f_int32":0e99999999999}', None), (A, b'{"f_uint64":"0e-99999999999"}', None),
     (A, b'{"f_int64":0e100000000,"f_sint32":0e-100000000}', None), (A, b'{"f_int64":0e100000001}', None),
     (A, b'{"r_double":[0e100000001,5e-100000001,0.0e00000000000000000000001]}', None),
+    (A, b'{"f_int32":0e2147483648,"f_uint64":"0.0e99999999999999999999","f_enum":-0e-99999999999}', None),
+    (A, b'{"r_int32":[1,0e200000000,-0.000e-2147483649]}', None), (A, b'{"f_int64":1e2147483648}', None),
+    # a quoted number that ends in a Unicode space (U+0085, U+00A0, U+2000-200A, U+3000, ...) fails strings.TrimSpace's
+    # check (found by the integer reference: only ASCII spaces were refused); any other character behind the number ends it
+    (A, b'{"f_int32":"1\\u00a0"}', None), (A, b'{"f_uint64":"7\\u3000"}', None), (A, b'{"r_int32":[1,"2\\u0085"]}', None),
+    (A, b'{"f_double":"1.5\\u2028"}', None), (A, b'{"f_sint64":"-3\\u200a"}', None), (A, b'{"f_int64":"1\\u00e9"}', None),
     # halfway points written exactly, and followed by a nonzero digit far behind the 40th significant one: 1 and the
     # next double up, 0 and the smallest float32 / double subnormal, DBL_MAX and 2^1024 (out of range above the tie)
     (A, b'{"f_double":1.00000000000000011102230246251565404236316680908203125}', None),
