@@ -246,9 +246,10 @@ GGR_DEV int parse_timestamp(StrIter& it, i64* secs, i32* nanos) {
   bool leap = (year % 4 == 0 && year % 100 != 0) || year % 400 == 0;
   if (mon == 2 && leap) maxd = 29;
   if (day < 1 || day > maxd) return GST_INVALID_VALUE;
-  if (frac_period && frac_digits > 9) return GST_INVALID_VALUE;
   i64 s = days_from_civil((i64)year, mon, day) * 86400 + (i64)(hh * 3600 + mi * 60 + ss) - off;
+  // protojson checks the seconds range before the length of a '.' fraction: out of range with a long fraction is RANGE
   if (s < -62135596800ll || s > 253402300799ll) return GST_RANGE;
+  if (frac_period && frac_digits > 9) return GST_INVALID_VALUE;
   *secs = s;
   *nanos = (i32)ns;
   return GST_OK;
@@ -711,6 +712,14 @@ GGR_DEVN int parse_scalar_at(EncCtx& cx, u32 pos, u32 kind, i32 child, Leaf* l, 
   return st;
 }
 
+// null as a list element or map value is a value like any other: protojson reads it as an unexpected token where a
+// message is due (Timestamp, Duration, FieldMask and Empty included) and as an invalid value where a scalar is, the bare
+// value of a wrapper too (unmarshalWrapperType reads the value field as a scalar)
+GGR_DEV int null_element_status(const Tables& T, const FieldD& f) {
+  if (f.kind != GK_MESSAGE) return GST_INVALID_VALUE;
+  return ggr_msg(T, (u32)f.child).wkt == GGR_WKT_WRAPPER ? GST_INVALID_VALUE : GST_SYNTAX;
+}
+
 // `active` is false for lanes that have no item (they only take part in the convergence votes);
 // `mask` names the lanes that call this function together.
 GGR_DEV int encode_parse(const Tables& T, u32 root_msg, const u8* in, u32 start, u32 end, u8* ir, u32 ir_cap, EncResult* res,
@@ -904,9 +913,9 @@ GGR_DEV int encode_parse(const Tables& T, u32 root_msg, const u8* in, u32 start,
         if (kf.kind == GK_STRING) node_store(ir, kidx, kl.a, kl.b, GGR_NIL, 0, node_meta(N_STR, kl.flags, kf.tag));
         else node_store(ir, kidx, (u32)map_key_val, (u32)(map_key_val >> 32), GGR_NIL, kf.kind, node_meta(kl.type, NF_RAWKEY, kf.tag));
         if (r.get() == 'n' ) {
-          // null map values are invalid for every value kind we support
+          // a null map value fails for every value kind
           if (!match_literal(r, LIT4('n', 'u', 'l', 'l'), 4, 0)) GGR_RET(GST_SYNTAX);
-          GGR_RET(f.kind == GK_MESSAGE ? GST_SYNTAX : GST_INVALID_VALUE);
+          GGR_RET(null_element_status(T, f));
         }
         want_value = true;
       }
@@ -926,7 +935,7 @@ GGR_DEV int encode_parse(const Tables& T, u32 root_msg, const u8* in, u32 start,
       f = ggr_field(T, fr.ref);
       if (r.get() == 'n') {
         if (!match_literal(r, LIT4('n', 'u', 'l', 'l'), 4, 0)) GGR_RET(GST_SYNTAX);
-        GGR_RET(f.kind == GK_MESSAGE ? GST_SYNTAX : GST_INVALID_VALUE);
+        GGR_RET(null_element_status(T, f));
       }
       want_value = true;
     }

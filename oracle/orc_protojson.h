@@ -431,8 +431,9 @@ static const int64_t kMinTs = -62135596800LL, kMaxTs = 253402300799LL;
 
 // time.Parse(time.RFC3339Nano, s) followed by protojson's own checks
 // [upstream encoding/protojson/well_known_types.go unmarshalTimestamp; time/format.go parse]
-// Accepts: YYYY-MM-DDTHH:MM:SS[(.|,)d+](Z|(+|-)HH:MM)
-inline bool parse_rfc3339(const Bytes& s, int64_t& secs, int32_t& nanos) {
+// Accepts: YYYY-MM-DDTHH:MM:SS[(.|,)d+](Z|(+|-)HH:MM).  *long_frac: a '.' fraction of more than 9 digits, which
+// protojson refuses only after its range check
+inline bool parse_rfc3339(const Bytes& s, int64_t& secs, int32_t& nanos, bool* long_frac) {
   size_t i = 0, n = s.size();
   auto dig = [&](size_t k) { return k < n && s[k] >= '0' && s[k] <= '9'; };
   auto fixed2 = [&](int& v) {  // getnum(value, true)
@@ -513,7 +514,7 @@ inline bool parse_rfc3339(const Bytes& s, int64_t& secs, int32_t& nanos) {
   nanos = (int32_t)ns;
   // protojson: a '.'-introduced subsecond field longer than ".999999999" is rejected
   // (LastIndexByte(s,'.') / LastIndexAny(s,"Z-+")); ','-introduced ones are truncated by time.Parse
-  if (frac_period && frac_digits > 9) return false;
+  *long_frac = frac_period && frac_digits > 9;
   return true;
 }
 // [upstream internal/strs JSONSnakeCase / JSONCamelCase, protoreflect FullName.IsValid]
@@ -729,8 +730,11 @@ struct PJUnmarshal {
     if (t.kind != K_STRING) return unexpected(t);
     int64_t secs;
     int32_t nanos;
-    if (!parse_rfc3339(t.str, secs, nanos)) return err.fail(ORC_INVALID_VALUE, "invalid google.protobuf.Timestamp value " + t.raw);
+    bool long_frac;
+    if (!parse_rfc3339(t.str, secs, nanos, &long_frac)) return err.fail(ORC_INVALID_VALUE, "invalid google.protobuf.Timestamp value " + t.raw);
+    // [upstream unmarshalTimestamp] the seconds range first, then the length of the subsecond field
     if (secs < kMinTs || secs > kMaxTs) return err.fail(ORC_RANGE, "google.protobuf.Timestamp value out of range: " + t.raw);
+    if (long_frac) return err.fail(ORC_INVALID_VALUE, "invalid google.protobuf.Timestamp value " + t.raw);
     Val a, b;
     a.u = (uint64_t)secs;
     b.u = (uint64_t)(int64_t)nanos;

@@ -140,6 +140,11 @@ ENCODE_EDGE = [
     (A, b'{"f_float":0.%s0001}' % str(5 ** 150).rjust(150, "0").encode(), None),
     (A, b'{"f_double":0.%s0001}' % str(5 ** 1075).rjust(1075, "0").encode(), None),
     (A, b'{"f_double":%d.0001,"f_int32":1}' % ((2 ** 54 - 1) << 970), None), (A, b'{"f_double":-%d}' % ((2 ** 54 - 1) << 970), None),
+    # found by the time reference: protojson checks a Timestamp's seconds range before the length of its '.' fraction (a
+    # range error, not an invalid value); null as a list element or map value of a wrapper is an invalid value (the
+    # wrapper reads its bare value as a scalar), not an unexpected token
+    (A, b'{"ts":"9999-12-31T23:59:59.1234567890-00:01"}', None), (A, b'{"r_ts":["0000-12-31T23:59:59.1234567890Z"]}', None),
+    (WK, b'{"r_i32":[1,null]}', None), (WK, b'{"m_i64":{"1":null}}', None), (WK, b'{"r_sv":[null]}', None),
 ]
 
 DECODE_EDGE_HEX = [
